@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- deep-image-prior hot path on B200: optimisation iterations/sec, 512x512 skip-net denoising.
+"""bench.py -- deep-image-prior hot path on H100: optimisation iterations/sec, 512x512 skip-net denoising.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
 
 A "step" is one optimisation iteration of BASELINE.json configs[1] (denoising F16-sized 512x512, skip[128x5], fp32):
@@ -11,14 +11,15 @@ One independent image per GPU (weak scaling, no data-path collective; NCCL only 
 Order of the run (our arm), all on the device clock (CUDA events), max over ranks:
   1. W warm-up steps, then ONE FULL IMAGE = 2000 iterations (BASELINE.json configs[0]/[1] budget, ~6 s): `image_run`
      and `images_per_sec` are MEASURED over it, with nvidia-smi clocks sampled throughout (sustained clocks);
-  2. immediately after, the K steps the driver asked for -> `value` / `ms_per_step` (clocks already in their sustained
-     state, inputs resident in HBM, closure-free device runner dip_run_iterations);
+  2. immediately after, the K steps asked for -> `value` / `ms_per_step` (clocks already in their sustained
+     state, inputs resident in HBM, closure-free device runner dip_run_iterations); --dump-outputs DIR writes what these
+     steps computed (out.npy, loss_hist.npy, params.npy);
   3. a short eager pass with CUDA events around every launch -> `roofline*` (algorithmic FLOPs or bytes / device time);
   4. `e2e`: utils.optimize('adam', params, closure, LR, n) with the notebook's closure (on-device noise.normal_() like
      denoising.ipynb c10:12-13, the step's input copied host(pinned)->device and the loss read back inside the region);
      `e2e_verbatim_closure`: the same with the verbatim c10 closure (EMA, 3 x PSNR read-backs, parameter snapshot);
   5. `gpu_library_baseline`: the SAME module tree executed by stock torch.cuda + cuDNN (cudnn.benchmark, TF32 default),
-     lean closure -- the reference's own GPU path on this B200 (BASELINE.md 3.4);
+     lean closure -- the reference's own GPU path on the same GPU (BASELINE.md 3.4);
   6. rank 0, N=1: `cpu_baseline` = the reference arm below on a bounded sample.
 --impl reference: the reference's CPU implementation of the same step on the host cores: the UNMODIFIED reference from
   oracle/_ref (copied by oracle/make_ref.py; kind "reference") when present, else the oracle port (kind "port").
@@ -41,7 +42,7 @@ SIGMA_REG = 1.0 / 30.0
 LR = 0.01
 ITERS_PER_IMAGE = 2000           # BASELINE.json configs[0]/[1]
 ALG_GFLOP_PER_ITER = 460.07      # SURVEY.md section 6 (2*M*N*K over the 26 convs, fwd+dgrad+wgrad)
-# dram__bytes_read.sum + dram__bytes_write.sum of the dominant launches from the committed `ncu --set full` captures
+# dram__bytes_read.sum + dram__bytes_write.sum of the dominant launches, when a capture is committed under profiles/
 TRAFFIC = json.load(open(os.path.join(ROOT, "profiles", "traffic.json"))) if os.path.exists(
     os.path.join(ROOT, "profiles", "traffic.json")) else {}
 METRIC = "optimisation iterations/sec (512x512 skip-net denoising, sum over independent images)"
@@ -57,7 +58,8 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p)), "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback (B200_PROFILING.md)"
+    # NVIDIA's H100 SXM data sheet (dense BF16; TF32 is half of it) -- an upper bound, not a rate this card has been seen to reach
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -319,10 +321,18 @@ def run_ours(args):
     img_ms, img_win = timed(lambda: device_steps(ITERS_PER_IMAGE, img_hist))
     with torch.no_grad():
         psnr_img = 10 * np.log10(1.0 / float(((out_buf.cpu() - clean_h) ** 2).mean()))
-    # ---- 2. `value`: the K steps the driver asked for, right behind the image (sustained clocks) -------------------
+    # ---- 2. `value`: the K steps asked for, right behind the image (sustained clocks) -------------------
     hist = torch.zeros(args.steps, dtype=torch.float64, device=dev)
     ms, val_win = timed(lambda: device_steps(args.steps, hist))
     value = mg.aggregate_rate(args.steps, ms / 1000.0, world)
+    if args.dump_outputs and rank == 0:
+        # what the timed steps hand back: the network output of the last step, the loss of every step and the parameters
+        # after the last Adam update (float32 / float64, ~13 MB); the inputs are seeded, so two builds compare value by value
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "out.npy"), out_buf.float().cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "loss_hist.npy"), hist.cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "params.npy"),
+                torch.cat([p.detach().reshape(-1) for p in params]).float().cpu().numpy())
 
     # ---- 3. roofline pass: CUDA events around every launch of a short eager pass (graphs cannot be event-bracketed) --
     roof_steps = min(args.steps, 10)
@@ -470,7 +480,7 @@ def run_ours(args):
         dist.barrier()
 
     # ---- 6. BASELINE configs[2]: super-resolution x4 (1024^2 net output -> 256^2 through the Lanczos-2 operator), runner,
-    #         in the default tf32 mode and in bf16 (tcgen05 kind::f16 on bf16 operands) -- single GPU, rank 0 only
+    #         in the default tf32 mode and in bf16 (wgmma on bf16 operands) -- single GPU, rank 0 only
     sr_cfg = None
     if rank == 0 and world == 1:
         del fast
@@ -515,12 +525,12 @@ def run_ours(args):
             d.update(extra or {})
             return d
 
-        note = ("peak = tf32 dense = 1/2 of the measured BURST bf16 cuBLAS rate (%s): the kernels are timed alone in a ~30 ms "
-                "pass, not inside a seconds-long tensor load; peak_sustained = 1/2 of the sustained rate" % peak_src)
-        roof = tensor_roof("tc_conv_kernel (tcgen05 tf32 implicit GEMM): ALL fprop + dgrad launches of a step",
+        note = ("peak = tf32 dense = 1/2 of the bf16 rate (%s); the kernels are timed alone in a ~30 ms pass; "
+                "peak_sustained = 1/2 of the sustained bf16 rate where one was measured" % peak_src)
+        roof = tensor_roof("tc_conv_kernel (wgmma tf32 implicit GEMM): ALL fprop + dgrad launches of a step",
                            lambda r: r[0] in (0, 1),
                            {"peak_note": note, "traffic": TRAFFIC.get("tc_conv_dominant"),
-                            "traffic_note": "dram read+write of the dominant launch (level-0 3x3 up conv fprop) from profiles/; null until captured for this kernel version",
+                            "traffic_note": "dram read+write of the dominant launch (level-0 3x3 up conv fprop) from profiles/; null until captured",
                             "timed": "CUDA events around every launch in a %d-step eager pass right after the timed region "
                                      "(side streams off so that kernels run alone)" % roof_steps})
         big = max(r[1] for r in records if r[0] == 0)
@@ -564,14 +574,14 @@ def run_ours(args):
             "gpu_library_baseline": {"value": lib_value, "unit": "it/s", "n_gpus": 1,
                                      "what": "the same module tree executed by stock torch.cuda + cuDNN (cudnn.benchmark=True, "
                                              "TF32 convolutions = torch default), lean closure, torch.optim.Adam -- the "
-                                             "reference's own GPU path on this B200 (denoising.ipynb c3:17-19)",
+                                             "reference's own GPU path on the same GPU (denoising.ipynb c3:17-19)",
                                      "speedup_value_per_gpu": (value / world) / lib_value if lib_value else None},
             "gpu_launches": int(launches_per_step * args.steps),
             "gpu_launches_per_step": int(launches_per_step),
             "roofline": roof,
             "roofline_dominant_launch": tensor_roof("tc_conv_kernel, level-0 3x3 conv 132->128 @512x512 fprop (largest launch)",
                                                     lambda r: r[0] == 0 and r[1] == big),
-            "roofline_wgrad": tensor_roof("tc_wgrad_kernel (tcgen05 tf32, MN-major operands, split-K), all launches",
+            "roofline_wgrad": tensor_roof("tc_wgrad_kernel (wgmma tf32, operands transposed in shared memory, split-K), all launches",
                                           lambda r: r[0] == 2),
             "roofline_hbm_all": hbm_roof("all HBM-bound launches of a step (sum of algorithmic bytes / sum of device time)",
                                          lambda r: r[0] >= 16, {"by_kernel": by_kernel}),
@@ -710,7 +720,11 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs writes what the engine's timed steps computed; the reference arm has no such outputs")
     if args.impl == "reference":
         run_reference(args)
     else:

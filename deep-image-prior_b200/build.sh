@@ -1,9 +1,9 @@
 #!/bin/bash
-# Builds libdip.so (sm_100a) in-tree. Usage: deep-image-prior_b200/build.sh
+# Builds libdip.so (sm_90a) in-tree. Usage: deep-image-prior_b200/build.sh
 set -e
 cd "$(dirname "$0")"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
-FLAGS="-O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -lineinfo -Xcompiler -fPIC --expt-relaxed-constexpr"
+FLAGS="-O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -Xcompiler -fPIC --expt-relaxed-constexpr"
 mkdir -p build
 for f in deep downsample conv_simt engine; do   # deep.cu contains conv_tc.cu + kernels_mem.cu (one translation unit)
   if [ ! -f build/$f.o ] || [ csrc/$f.cu -nt build/$f.o ] || { [ $f = deep ] && { [ csrc/conv_tc.cu -nt build/deep.o ] || [ csrc/kernels_mem.cu -nt build/deep.o ]; }; } || [ -n "$(find csrc include ../include -name '*.h' -newer build/$f.o -o -name '*.cuh' -newer build/$f.o 2>/dev/null)" ]; then

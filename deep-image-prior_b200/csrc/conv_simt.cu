@@ -1,4 +1,4 @@
-// Exact-fp32 CUDA-core convolutions (precision mode "fp32"): same operand layouts and semantics as the tcgen05
+// Exact-fp32 CUDA-core convolutions (precision mode "fp32"): same operand layouts and semantics as the wgmma
 // kernels in conv_tc.cu, FMA arithmetic in IEEE fp32.  Used for the parity tier that must not see TF32 rounding
 // (SURVEY.md section 7.4, P2) and as the on-device cross-check of the tensor-core path.
 // Reference semantics: torch.nn.Conv2d forward / backward (models/common.py:120).

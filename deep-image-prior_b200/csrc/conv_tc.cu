@@ -1,25 +1,27 @@
-// tcgen05 / TMA implicit-GEMM convolution kernels for sm_100a (hand-written, no CUTLASS).
+// wgmma / TMA implicit-GEMM convolution kernels for sm_90a (hand-written, no CUTLASS).
 //
 // Replaces what torch.nn.Conv2d forward/backward computes for the skip network
 // (reference call site: models/common.py:120 via models/skip.py:58,64,68,83,89; backward = autograd of same).
 //
-//   tc_conv_kernel  : fprop and dgrad.  Persistent, warp-specialised:
+//   tc_conv_kernel  : fprop and dgrad.  Persistent, warp-specialised, 256 threads:
 //                       warp 0     TMA producer (im2col folded into the tensor-map coordinates: one 5-D box per tap)
-//                       warp 1     single-thread tcgen05.mma issuer, fp32 accumulators in TMEM (double-buffered)
-//                       warp 2     TMEM allocator
-//                       warps 4-7  epilogue: tcgen05.ld -> +bias -> swizzled smem -> per-channel BN statistics
-//                                  -> TMA store
-//   tc_wgrad_kernel : weight gradient, both operands MN-major straight from NHWC activations, split-K over CTAs.
-//   Both are templated on the operand type: kind::tf32 on fp32 tensors (tc_conv_kernel / tc_wgrad_kernel) and kind::f16 on
-//   bf16 twins (tc_conv_kernel_bf16 / tc_wgrad_kernel_bf16, precision mode bf16); accumulators and outputs are fp32 in both.
+//                       warp 3     loads the bias
+//                       warps 4-7  one warpgroup: wgmma on the 128-pixel tile (two m64 halves, fp32 accumulators in
+//                                  registers), then the epilogue: +bias -> swizzled smem -> per-channel BN statistics -> TMA store
+//   tc_wgrad_kernel : weight gradient, split-K over work items (tap, pixel range), one partial slice per item.  dY and X arrive pixel-major from NHWC
+//                     activations; wgmma reads tf32 operands K-major only, so the warpgroup transposes each stage into
+//                     K-major 128-byte-swizzled tiles (double-buffered) before it multiplies.
+//   Both are templated on the operand type: tf32 on fp32 tensors (tc_conv_kernel / tc_wgrad_kernel) and bf16 on bf16 twins
+//   (tc_conv_kernel_bf16 / tc_wgrad_kernel_bf16, precision mode bf16); accumulators and outputs are fp32 in both.
 #include "conv_tc.cuh"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 #include "kernels.cuh"
 
 namespace dip {
 
-static constexpr int kTileM = 128;            // output pixels per tile (UMMA M)
-static constexpr int kABytes = kTileM * 128;  // one A stage: 128 rows x 32 fp32
+static constexpr int kTileM = 128;            // output pixels per tile (two wgmma m64 halves)
+static constexpr int kABytes = kTileM * 128;  // one A stage: 128 rows x 128 bytes
 static constexpr int kChunkBytes = kTileM * 128;
 static constexpr int kNumThreads = 256;
 static constexpr int kAccStride = kAccS;  // fp64 accumulators: kAccR replicas x one 128-byte line each (kernels.cuh)
@@ -27,79 +29,172 @@ static constexpr int kAccStride = kAccS;  // fp64 accumulators: kAccR replicas x
 struct SmemCtl {
   uint64_t full[8];
   uint64_t empty[8];
-  uint64_t tmem_full[4];   // one per TMEM accumulator buffer: 2 (single tiles, double-buffered), 4 or 3 (tile pairs)
-  uint64_t tmem_empty[4];
-  uint64_t a_full[2];    // patch mode: input patch buffers
-  uint64_t a_empty[2];
-  uint32_t tmem_base;
-  uint32_t pad;
   float bias[160];
 };
 
-__device__ __forceinline__ uint32_t tmem_cols_pow2(uint32_t n) {
-  uint32_t c = 32;
-  while (c < n) c <<= 1;
-  return c;
-}
+__host__ __device__ constexpr int round32(int n) { return (n + 31) & ~31; }
+__host__ __device__ constexpr int round1024(int n) { return (n + 1023) & ~1023; }
 
 // ------------------------------------------------------------------------------------------------ fprop / dgrad
+// Consumer warpgroup (threads 128..255) of the conv kernel, NT = wgmma N (n_mma rounded up to 32).
+template <bool BF16, int NT>
+__device__ __forceinline__ void tc_conv_consumer(const TcConvParams& p, const TcConvParams* pm, SmemCtl* ctl,
+                                                 uint8_t* stage_base, int stage_bytes, uint8_t* staging, int n_iters,
+                                                 int tile0, int tile_stride, int num_tiles, int tiles_pp, int n_off) {
+  const int et = threadIdx.x - 128;    // 0..127
+  const int w = et >> 5, lane = et & 31;
+  float acc[2][NT / 2];
+  int stage = 0;
+  uint32_t phase = 0;
+  double stat_s1 = 0.0, stat_s2 = 0.0;
+  const int bw_shift = 31 - __clz(p.bw);  // tile widths are powers of two
+  const uint32_t base_lo = desc_lo(smem_u32(stage_base));
+  const uint32_t stage_step = static_cast<uint32_t>(stage_bytes) >> 4;
+  constexpr uint32_t kBOff = static_cast<uint32_t>(kABytes) >> 4;
+  constexpr uint32_t kHalfOff = (64u * 128u) >> 4;   // second m64 half of the A tile
+  for (int it = 0; it < n_iters; ++it) {
+    const int tile = tile0 + it * tile_stride;
+    int tx = tile % p.tiles_x, ty = tile / p.tiles_x;
+    int opx = 0, opy = 0;
+    int kb_per_tile = p.kh * p.kw * p.kblocks;
+    if (p.nphase > 0) {
+      if (tile >= num_tiles) break;
+      const int t = tile % tiles_pp;
+      tx = t % p.tiles_x; ty = t / p.tiles_x;
+      const TcConvParams::Phase& q = p.phs[tile / tiles_pp];
+      opx = q.opx; opy = q.opy;
+      kb_per_tile = q.kh * q.kw * p.kblocks;
+    }
+    const int x0 = tx * p.bw, y0 = ty * p.bh;
+#pragma unroll
+    for (int i = 0; i < NT / 2; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
+    int prev = -1;
+    for (int kbt = 0; kbt < kb_per_tile; ++kbt) {
+      mbar_wait(&ctl->full[stage], phase);
+      const uint32_t a_lo = base_lo + stage * stage_step;
+      const uint32_t b_lo = a_lo + kBOff;
+      // all four K steps of every block: channels past C are zero in both operands (TMA zero-fills the activation past
+      // its channel extent, the packed weights are zero there), so a partial last block needs no shorter issue sequence
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {   // K-major SW128: advancing K by 8 fp32 / 16 bf16 = +32 B inside the swizzle atom
+        wgmma_ss<NT, BF16>(acc[0], desc_of(a_lo + 2 * k), desc_of(b_lo + 2 * k));
+        wgmma_ss<NT, BF16>(acc[1], desc_of(a_lo + kHalfOff + 2 * k), desc_of(b_lo + 2 * k));
+      }
+      wgmma_commit();
+      if (prev >= 0) {   // the previous stage's wgmmas have read their operands -> hand it back to the producer
+        wgmma_wait<1>();
+        if (lane == 0) mbar_arrive(&ctl->empty[prev]);
+      }
+      prev = stage;
+      if (++stage == p.stages) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    if (prev >= 0 && lane == 0) mbar_arrive(&ctl->empty[prev]);
+
+    // staging buffer must be free (previous tile's TMA store has finished reading it)
+    if (et == 0) tma_store_wait_read0();
+    named_bar_sync(1, 128);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int j = 0; j < NT / 8; ++j) {
+        const int col = 8 * j + 2 * (lane & 3);
+        const int chunk = col >> 5;
+        if (chunk < p.n_chunks) {
+          const int q = (col & 31) >> 2, e = col & 3;
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr) {
+            const int row = 64 * h + 16 * w + (lane >> 2) + 8 * rr;
+            float2 o;
+            o.x = acc[h][4 * j + 2 * rr] + ctl->bias[col];
+            o.y = acc[h][4 * j + 2 * rr + 1] + ctl->bias[col + 1];
+            *reinterpret_cast<float2*>(staging + chunk * kChunkBytes + row * 128 + ((q ^ (row & 7)) << 4) + e * 4) = o;
+          }
+        }
+      }
+    }
+    fence_proxy_async_smem();
+    named_bar_sync(1, 128);
+    if (et == 0) {
+      if (p.nphase > 0)
+        for (int j = 0; j < p.n_chunks; ++j) tma_store_5d(&pm->tmD, staging + j * kChunkBytes, n_off + j * 32, opx, x0, opy, y0);
+      else
+        for (int j = 0; j < p.n_chunks; ++j) tma_store_3d(&pm->tmD, staging + j * kChunkBytes, n_off + j * 32, x0, y0);
+      tma_store_commit();
+    }
+    if (p.stats != nullptr && et < p.n_mma) {
+      // per-channel sum / sum-of-squares of this tile (feeds the following BatchNorm): thread = channel et, running
+      // totals stay in registers across all tiles of this persistent CTA (one fp64 atomic pair per thread at the end)
+      const int c = et;
+      const int j = c >> 5, q = (c & 31) >> 2, e = c & 3;
+      const uint8_t* cb = staging + j * kChunkBytes + e * 4;
+      float a0 = 0.f, a1 = 0.f, b0 = 0.f, b1 = 0.f;
+      if (x0 + p.bw <= p.out_w && y0 + p.bh <= p.out_h) {
+#pragma unroll 8
+        for (int m = 0; m < kTileM; m += 2) {
+          const float x = *reinterpret_cast<const float*>(cb + m * 128 + ((q ^ (m & 7)) << 4));
+          const float y = *reinterpret_cast<const float*>(cb + (m + 1) * 128 + ((q ^ ((m + 1) & 7)) << 4));
+          a0 += x; b0 = fmaf(x, x, b0);
+          a1 += y; b1 = fmaf(y, y, b1);
+        }
+      } else {
+        for (int m = 0; m < kTileM; ++m) {
+          const int py = m >> bw_shift, px = m & (p.bw - 1);
+          if (x0 + px < p.out_w && y0 + py < p.out_h) {
+            const float x = *reinterpret_cast<const float*>(cb + m * 128 + ((q ^ (m & 7)) << 4));
+            a0 += x; b0 = fmaf(x, x, b0);
+          }
+        }
+      }
+      stat_s1 += static_cast<double>(a0 + a1);
+      stat_s2 += static_cast<double>(b0 + b1);
+    }
+  }
+  if (p.stats != nullptr && et < p.n_mma && n_off + et < p.stats_ld) {
+    const int rep = (blockIdx.x % kAccR) * kAccLine;
+    atomicAdd(&p.stats[(n_off + et) * kAccStride + rep], stat_s1);
+    atomicAdd(&p.stats[(p.stats_ld + n_off + et) * kAccStride + rep], stat_s2);
+  }
+  if (et == 0) tma_store_wait_all0();
+}
+
 // Body of the conv kernel.  DEEP = false: the stand-alone launch (tc_conv_kernel).  DEEP = true: one PHASE of the persistent
 // deep-level kernel (deep.cu): `p` is a shared-memory copy of the scalars, `pm` the parameter block in global memory whose
-// tensor maps TMA reads; TMEM (512 columns) is allocated once by the caller and handed in as tmem_pre; the CTA-local
-// barriers are re-initialised here (every barrier of the previous phase has completed all its phases by then); CTAs
-// beyond the grid the stand-alone launch would have used (p.vgrid) sit the phase out.
-// BF16 = true: operands are bf16 (kind::f16, K = 16 per MMA).  The BYTE geometry is unchanged -- an operand row is still
-// 128 bytes, now 64 channels, and one MMA still advances 32 bytes along K -- so a "k block" is 64 channels, p.kblocks /
-// p.tail_mmas count those, and only the channel coordinate of the TMA boxes and the instruction kind differ.
+// tensor maps TMA reads; the CTA-local barriers are re-initialised here (every barrier of the previous phase has completed
+// all its phases by then); CTAs beyond the grid the stand-alone launch would have used (p.vgrid) sit the phase out.
+// BF16 = true: operands are bf16 (K = 16 per wgmma).  The BYTE geometry is unchanged -- an operand row is still 128 bytes,
+// now 64 channels, and one wgmma still advances 32 bytes along K -- so a "k block" is 64 channels, p.kblocks counts
+// those, and only the channel coordinate of the TMA boxes and the instruction type differ.
 template <bool DEEP, bool BF16 = false>
-__device__ __forceinline__ void tc_conv_body(const TcConvParams& p, const TcConvParams* pm, uint8_t* smem_raw, uint32_t tmem_pre) {
+__device__ __forceinline__ void tc_conv_body(const TcConvParams& p, const TcConvParams* pm, uint8_t* smem_raw) {
   constexpr int KE = BF16 ? 64 : 32;   // channels per 128-byte operand row
   const int grid_x = DEEP ? p.vgrid : static_cast<int>(gridDim.x);
   if (DEEP && static_cast<int>(blockIdx.x) >= grid_x) return;
   // 1024-byte alignment is required by the 128B swizzle atoms.
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int b_bytes = p.n_mma * 128;
-  // per-tap mode: stage = [A tile 16 KB][B tile]; patch mode: two input patches up front, stages hold B tiles only
-  const int patch_bytes = p.patch ? p.pw * p.ph * 128 : 0;
-  const int patch_alloc = (patch_bytes + 127) & ~127;
-  const int tps = p.patch ? p.tps : 1;  // filter taps per B stage (patch mode)
-  const int stage_bytes = (p.patch ? 0 : kABytes) + ((tps * b_bytes + 1023) & ~1023);
-  // layout: [weight (+A) stages | epilogue staging | 2 input patches | control].  Stages and staging are 1024-byte aligned
-  // (swizzle atoms); the patches only need 128 bytes: TMA and UMMA both swizzle on absolute smem address bits.
+  const int nt = round32(p.n_mma);
+  const int b_bytes = p.n_mma * 128;                       // bytes TMA writes per B tile
+  const int stage_bytes = kABytes + round1024(nt * 128);   // [A tile 16 KB][B tile, room for nt rows]
+  // layout: [stages | epilogue staging | control], stages and staging 1024-byte aligned (swizzle atoms)
   uint8_t* stage_base = smem;
   uint8_t* staging = stage_base + p.stages * stage_bytes;
-  const int pair = p.pair;                                  // two tiles per iteration (see TcConvParams::pair)
-  const int stg_chunks = pair ? 2 : p.n_chunks;             // pair mode stores a tile 64 channels at a time
-  uint8_t* patch_base = staging + stg_chunks * kChunkBytes;
-  SmemCtl* ctl = reinterpret_cast<SmemCtl*>(patch_base + 2 * patch_alloc);
+  SmemCtl* ctl = reinterpret_cast<SmemCtl*>(staging + p.n_chunks * kChunkBytes);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int tiles_pp = p.tiles_x * p.tiles_y;                     // tiles per sub-pixel phase (nphase > 0)
-  const int num_tiles = p.pair ? p.tiles_x * ((p.tiles_y + 1) / 2)   // pair mode: work items are tile pairs
-                               : p.nphase > 0 ? tiles_pp * p.nphase : tiles_pp;
-  // Cluster of `csize` CTAs: every CTA works on its own tile, all of them walk the identical (tap, k-block) sequence, and
-  // each CTA fetches 1/csize of the weight tile and multicasts it to the whole cluster (weights are the same for all
-  // tiles) -> L2->SM traffic per k-block drops from 16+16 KB to 16+16/csize KB.  Tiles past the end are harmless
-  // dummies (TMA zero-fills out-of-range reads and clips out-of-range stores; statistics are masked).
-  const int csize = p.csize;
-  const uint32_t crank = csize > 1 ? cluster_ctarank() : 0u;
-  const uint16_t cmask = static_cast<uint16_t>((1u << csize) - 1u);
+  const int num_tiles = p.nphase > 0 ? tiles_pp * p.nphase : tiles_pp;
   // N split (small levels, fewer tiles than SMs): n_split CTAs share a pixel tile, each computes n_mma = N / n_split
-  // output channels -> each CTA ingests 1/n_split of the weights (per-SM ingest is what bounds a lone tile) and the
-  // tile's work spreads over more SMs.  CTA = (tile slot, n_part); n_split == 1: slots == gridDim.x.
+  // output channels -> each CTA ingests 1/n_split of the weights and the tile's work spreads over more SMs.
+  // CTA = (tile slot, n_part); n_split == 1: slots == gridDim.x.
   const int n_split = p.n_split < 1 ? 1 : p.n_split;
   const int n_part = blockIdx.x % n_split;
   const int n_off = n_part * p.n_mma;             // first output channel of this CTA
   const int n_total = p.n_mma * n_split;          // rows per tap of the packed weights
   const int tile_stride = grid_x / n_split;
   const int n_iters = (num_tiles + tile_stride - 1) / tile_stride;
-  const int tile0 = n_split > 1 ? blockIdx.x / n_split : (blockIdx.x / csize) * csize + crank;  // first tile; stride tile_stride
-  const uint32_t tile_cols = (p.n_mma + 31) & ~31;              // TMEM columns of one tile's accumulator
-  const uint32_t acc_cols = tile_cols;                          // column stride between accumulator buffers
-  // pair mode: accumulator buffers are handed out per TILE in round-robin order -- 4 buffers of 128 columns (two pairs in
-  // flight), or 3 of 160 (the 132-channel dgrad: the upper tile of the next pair reuses the buffer the epilogue drains first)
-  const int nbuf = pair ? (tile_cols * 4 <= 512 ? 4 : 3) : 2;
+  const int tile0 = blockIdx.x / n_split;         // first tile; stride tile_stride
 
   if (!DEEP) pdl_trigger();
   if (warp == 0 && lane == 0) {
@@ -110,518 +205,191 @@ __device__ __forceinline__ void tc_conv_body(const TcConvParams& p, const TcConv
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < p.stages; ++i) {
       mbar_init(&ctl->full[i], 1);
-      mbar_init(&ctl->empty[i], csize);  // released by the MMA warp of every CTA that multicasts into this stage
-    }
-    for (int i = 0; i < 4; ++i) {
-      mbar_init(&ctl->tmem_full[i], 1);
-      mbar_init(&ctl->tmem_empty[i], 4);  // one arrival per epilogue warp
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&ctl->a_full[i], 1);
-      mbar_init(&ctl->a_empty[i], 1);
+      mbar_init(&ctl->empty[i], 4);   // one arrival per consumer warp
     }
     fence_mbar_init();
-  }
-  if (!DEEP && warp == 2) {
-    tmem_alloc(&ctl->tmem_base, tmem_cols_pow2(nbuf * acc_cols));
-    tmem_relinquish();
   }
   if (!DEEP) pdl_wait();  // everything above is independent of the previous kernel's results
   if (warp == 3) {
     for (int i = lane; i < 160; i += 32)
       ctl->bias[i] = (p.bias != nullptr && i < p.n_mma && (p.n_valid == 0 || n_off + i < p.n_valid)) ? p.bias[n_off + i] : 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  if (csize > 1) cluster_sync_all();  // peers' barriers must be initialised before any multicast / remote arrive
-  tc_fence_after();
-  const uint32_t tmem_base = DEEP ? tmem_pre : ctl->tmem_base;
 
   if (warp == 0) {
     // ===================================================================== TMA producer
-    // The whole warp walks the loop (warp-uniform control flow and addresses stay in uniform registers); one elected
-    // lane issues the TMA instructions.
-    {
-      int stage = 0;
-      uint32_t phase = 0;
-      const int b_rows = p.n_mma / csize;
-      int ab = 0;
-      uint32_t aphase = 0;
-      for (int it = 0; it < n_iters; ++it) {
-        const int tile = tile0 + it * tile_stride;
-        const int tx = tile % p.tiles_x, ty = tile / p.tiles_x;
-        const int x0 = tx * p.bw, y0 = ty * p.bh * (pair ? 2 : 1);
-        if (p.patch) {
-          // 3x3 stride-1: ONE (bw+2) x (bh+2) input patch per 32-channel block serves all nine taps (the MMA warp
-          // addresses tap (r,s) as the same patch shifted by r*pw+s rows); only the weight tiles stream per tap.
-          const int taps = p.kh * p.kw;
-          for (int kb = 0; kb < p.kblocks; ++kb) {
-            mbar_wait(&ctl->a_empty[ab], aphase ^ 1);
-            if (elect_one()) {
-              if (p.dbg_flags & 1) mbar_arrive(&ctl->a_full[ab]);
-              else {
-                mbar_expect_tx(&ctl->a_full[ab], patch_bytes);
-                tma_load_5d(patch_base + ab * patch_alloc, &pm->tmA, &ctl->a_full[ab], kb * KE, 0, x0 + p.offx, 0, y0 + p.offy);
-              }
-            }
-            __syncwarp();
-            if (++ab == 2) { ab = 0; aphase ^= 1; }
-            for (int tap = 0; tap < taps; tap += tps) {
-              if (p.dbg_flags & (64 | 128)) { if (++stage == p.stages) { stage = 0; phase ^= 1; } continue; }
-              mbar_wait(&ctl->empty[stage], phase ^ 1);
-              uint8_t* sb = stage_base + stage * stage_bytes;
-              if (elect_one()) {
-                if (p.dbg_flags & 2) mbar_arrive(&ctl->full[stage]);
-                else {
-                  // one box per tap; a box past the last tap is out of range -> zero-filled, never read
-                  mbar_expect_tx(&ctl->full[stage], tps * b_bytes);
-                  if (csize == 1) {
-                    for (int t = 0; t < tps; ++t)
-                      tma_load_2d(sb + t * b_bytes, &pm->tmB, &ctl->full[stage], kb * KE, (tap + t) * n_total + n_off);
-                  } else {
-                    tma_load_2d_mc(sb + crank * b_rows * 128, &pm->tmB, &ctl->full[stage], kb * KE,
-                                   tap * p.n_mma + crank * b_rows, cmask);
-                  }
-                }
-              }
-              __syncwarp();
-              if (++stage == p.stages) { stage = 0; phase ^= 1; }
-            }
-          }
-          continue;
-        }
-        // per-tap mode: one phase (kh x kw taps at offx / offy) or the phase this work item belongs to
-        int kh = p.kh, kw = p.kw, offx = p.offx, offy = p.offy, tap0 = 0, px0 = x0, py0 = y0;
-        if (p.nphase > 0) {
-          if (tile >= num_tiles) break;
-          const TcConvParams::Phase& q = p.phs[tile / tiles_pp];
-          const int t = tile % tiles_pp;
-          kh = q.kh; kw = q.kw; offx = q.offx; offy = q.offy; tap0 = q.tap0;
-          px0 = (t % p.tiles_x) * p.bw; py0 = (t / p.tiles_x) * p.bh;
-        }
-        for (int r = 0; r < kh; ++r) {
-          for (int s = 0; s < kw; ++s) {
-            const int ix = offx + s, iy = offy + r;  // tap offset in input coordinates
-            const int x0 = px0, y0 = py0;
-            int cpx, cx, cpy, cy;
-            if (p.stride == 1) {
-              cpx = 0; cx = x0 + ix; cpy = 0; cy = y0 + iy;
-            } else {
-              // input coordinate = 2*out + i  ->  (parity, half) = (i & 1, out + (i >> 1)); offsets are >= 0 here
-              cpx = ix & 1; cx = x0 + (ix >> 1); cpy = iy & 1; cy = y0 + (iy >> 1);
-            }
-            const int tap = tap0 + r * kw + s;
-            for (int kb = 0; kb < p.kblocks; ++kb) {
-              mbar_wait(&ctl->empty[stage], phase ^ 1);
-              uint8_t* sa = stage_base + stage * stage_bytes;
-              uint8_t* sb = sa + kABytes;
-              if (elect_one()) {
-                const bool ldA = !(p.dbg_flags & 1), ldB = !(p.dbg_flags & 2);
-                if (ldA || ldB) mbar_expect_tx(&ctl->full[stage], (ldA ? kABytes : 0) + (ldB ? b_bytes : 0));
-                else mbar_arrive(&ctl->full[stage]);
-                if (ldA) tma_load_5d(sa, &pm->tmA, &ctl->full[stage], kb * KE, cpx, cx, cpy, cy);
-                if (ldB) {
-                  if (csize == 1) tma_load_2d(sb, &pm->tmB, &ctl->full[stage], kb * KE, tap * n_total + n_off);
-                  else tma_load_2d_mc(sb + crank * b_rows * 128, &pm->tmB, &ctl->full[stage], kb * KE,
-                                      tap * p.n_mma + crank * b_rows, cmask);
-                }
-              }
-              __syncwarp();
-              if (++stage == p.stages) { stage = 0; phase ^= 1; }
-            }
-          }
-        }
+    // The whole warp walks the loop (warp-uniform control flow); one elected lane issues the TMA instructions.
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int it = 0; it < n_iters; ++it) {
+      const int tile = tile0 + it * tile_stride;
+      // one phase (kh x kw taps at offx / offy) or the phase this work item belongs to
+      int kh = p.kh, kw = p.kw, offx = p.offx, offy = p.offy, tap0 = 0;
+      int x0 = (tile % p.tiles_x) * p.bw, y0 = (tile / p.tiles_x) * p.bh;
+      if (p.nphase > 0) {
+        if (tile >= num_tiles) break;
+        const TcConvParams::Phase& q = p.phs[tile / tiles_pp];
+        const int t = tile % tiles_pp;
+        kh = q.kh; kw = q.kw; offx = q.offx; offy = q.offy; tap0 = q.tap0;
+        x0 = (t % p.tiles_x) * p.bw; y0 = (t / p.tiles_x) * p.bh;
       }
-    }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer
-    // One thread; its instruction stream is the critical path (a lone warp issues a dependent instruction only every
-    // few cycles), so the loop is kept minimal: descriptors are (lo, hi) 32-bit pairs, K advances by adding 2 to lo.
-    // All 32 lanes run the (warp-uniform) loop; one elected lane issues the MMAs and the commits.
-    {
-      const uint32_t idesc = BF16 ? make_idesc_bf16(kTileM, p.n_mma, 0, 0) : make_idesc_tf32(kTileM, p.n_mma, 0, 0);
-      const uint32_t bhi = desc_hi(1024, 2);
-      const uint32_t stage_lo0 = desc_lo(smem_u32(stage_base) + (p.patch ? 0 : kABytes), 16);
-      const uint32_t stage_lo_step = static_cast<uint32_t>(stage_bytes) >> 4;
-      const bool skip_mma = (p.dbg_flags & 8) != 0;
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      int ab = 0;
-      uint32_t aphase = 0;
-      for (int it = 0; it < n_iters; ++it) {
-        int kb_per_tile = p.kh * p.kw * p.kblocks;
-        if (p.nphase > 0) {
-          const int tile = tile0 + it * tile_stride;
-          if (tile >= num_tiles) break;
-          kb_per_tile = p.phs[tile / tiles_pp].kh * p.phs[tile / tiles_pp].kw * p.kblocks;
-        }
-        // accumulator buffers of this iteration: single tiles alternate between two; a pair takes the next two of nbuf
-        const int g0 = 2 * it;
-        const int b0 = pair ? g0 % nbuf : acc, b1 = (g0 + 1) % nbuf;
-        if (pair) {
-          mbar_wait(&ctl->tmem_empty[b0], (((g0 / nbuf) & 1) ^ 1));
-          mbar_wait(&ctl->tmem_empty[b1], ((((g0 + 1) / nbuf) & 1) ^ 1));
-        } else {
-          mbar_wait(&ctl->tmem_empty[acc], acc_phase ^ 1);
-        }
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + b0 * acc_cols;
-        uint32_t accf = 0;  // 0 for the first MMA of the tile (overwrite), 1 afterwards
-        if (p.patch) {
-          // tile row ty = 8 consecutive patch pixels starting at ((ty + r) * pw + sx): 8-row groups pw*128 B apart.  The
-          // group starts are not 1024 B aligned: UMMA and TMA both swizzle on absolute smem address bits (verified
-          // by scripts/exp_desc_shift.py), so a tap is just an address offset into the patch.
-          const uint32_t ahi = desc_hi(p.pw * 128, 2);
-          const uint32_t row_step = static_cast<uint32_t>(p.pw) * 8;  // one patch row, in 16-byte units
-          const uint32_t pair_off = row_step * static_cast<uint32_t>(p.bh);   // second tile of a pair: bh patch rows further down
-          const uint32_t tmem_d1 = tmem_base + b1 * acc_cols;
-          for (int kb = 0; kb < p.kblocks; ++kb) {
-            mbar_wait(&ctl->a_full[ab], aphase);
-            tc_fence_after();
-            uint32_t row_lo = desc_lo(smem_u32(patch_base + ab * patch_alloc), 16);
-            const int nmma = p.dbg_nmma ? p.dbg_nmma : ((kb == p.kblocks - 1) ? p.tail_mmas : 4);
-            const int taps = p.kh * p.kw;
-            const uint32_t tap_lo_step = static_cast<uint32_t>(b_bytes) >> 4;  // next tap inside a B stage
-            int sx = 0;
-            for (int tap = 0; tap < taps; tap += tps) {
-              if (!(p.dbg_flags & 128)) mbar_wait(&ctl->full[stage], phase);
-              if (!(p.dbg_flags & 32)) tc_fence_after();
-              const uint32_t b_lo = stage_lo0 + stage * stage_lo_step;
-              // A operand of tap (r, sx): the patch shifted by r rows and sx pixels; up to 3 taps share this round
-              const int nt = min(tps, taps - tap);
-              uint32_t a_lo[3];
-#pragma unroll
-              for (int t = 0; t < 3; ++t) {
-                a_lo[t] = row_lo + sx * 8;
-                if (t < nt && ++sx == p.kw) { sx = 0; row_lo += row_step; }
-              }
-              if (elect_one()) {
-                if (!skip_mma || accf == 0) {
-                  if (nmma == 4) {
-#pragma unroll
-                    for (int t = 0; t < 3; ++t) {
-                      if (t < nt) {
-                        const uint32_t bt = b_lo + t * tap_lo_step;
-                        mma_lohi<BF16>(tmem_d, a_lo[t], ahi, bt, bhi, idesc, t == 0 ? accf : 1u);
-                        mma_lohi<BF16>(tmem_d, a_lo[t] + 2, ahi, bt + 2, bhi, idesc, 1u);
-                        mma_lohi<BF16>(tmem_d, a_lo[t] + 4, ahi, bt + 4, bhi, idesc, 1u);
-                        mma_lohi<BF16>(tmem_d, a_lo[t] + 6, ahi, bt + 6, bhi, idesc, 1u);
-                        if (pair) {   // same weight tile, the lower tile of the pair
-                          const uint32_t a1 = a_lo[t] + pair_off;
-                          mma_lohi<BF16>(tmem_d1, a1, ahi, bt, bhi, idesc, t == 0 ? accf : 1u);
-                          mma_lohi<BF16>(tmem_d1, a1 + 2, ahi, bt + 2, bhi, idesc, 1u);
-                          mma_lohi<BF16>(tmem_d1, a1 + 4, ahi, bt + 4, bhi, idesc, 1u);
-                          mma_lohi<BF16>(tmem_d1, a1 + 6, ahi, bt + 6, bhi, idesc, 1u);
-                        }
-                      }
-                    }
-                  } else {
-                    for (int t = 0; t < nt; ++t)
-                      for (int k = 0; k < nmma; ++k) {
-                        mma_lohi<BF16>(tmem_d, a_lo[t] + 2 * (k & 3), ahi, b_lo + t * tap_lo_step + 2 * (k & 3), bhi, idesc,
-                                      (t | k) > 0 ? 1u : accf);
-                        if (pair)
-                          mma_lohi<BF16>(tmem_d1, a_lo[t] + pair_off + 2 * (k & 3), ahi, b_lo + t * tap_lo_step + 2 * (k & 3), bhi,
-                                        idesc, (t | k) > 0 ? 1u : accf);
-                      }
-                  }
-                }
-                if (!(p.dbg_flags & 64)) {
-                  if (csize == 1) tc_commit(&ctl->empty[stage]); else tc_commit_mc(&ctl->empty[stage], cmask);
-                }
-              }
-              __syncwarp();
-              accf = 1u;
-              if (++stage == p.stages) { stage = 0; phase ^= 1; }
-            }
-            if (elect_one()) tc_commit(&ctl->a_empty[ab]);
-            __syncwarp();
-            if (++ab == 2) { ab = 0; aphase ^= 1; }
+      for (int r = 0; r < kh; ++r) {
+        for (int s = 0; s < kw; ++s) {
+          const int ix = offx + s, iy = offy + r;  // tap offset in input coordinates
+          int cpx, cx, cpy, cy;
+          if (p.stride == 1) {
+            cpx = 0; cx = x0 + ix; cpy = 0; cy = y0 + iy;
+          } else {
+            // input coordinate = 2*out + i  ->  (parity, half) = (i & 1, out + (i >> 1)); offsets are >= 0 here
+            cpx = ix & 1; cx = x0 + (ix >> 1); cpy = iy & 1; cy = y0 + (iy >> 1);
           }
-        } else {
-          const uint32_t ahi = desc_hi(1024, 2);
-          const uint32_t a_off = stage_lo0 - (kABytes >> 4) + ((static_cast<uint32_t>(p.dbg_shift) * 128) >> 4);
-          int kb = 0;
-          for (int kbt = 0; kbt < kb_per_tile; ++kbt) {
-            mbar_wait(&ctl->full[stage], phase);
-            tc_fence_after();
-            const uint32_t a_lo = a_off + stage * stage_lo_step;
-            const uint32_t b_lo = stage_lo0 + stage * stage_lo_step;
-            const int nmma = (kb == p.kblocks - 1) ? p.tail_mmas : 4;
-            if (++kb == p.kblocks) kb = 0;
+          const int tap = tap0 + r * kw + s;
+          for (int kb = 0; kb < p.kblocks; ++kb) {
+            mbar_wait(&ctl->empty[stage], phase ^ 1);
+            uint8_t* sa = stage_base + stage * stage_bytes;
             if (elect_one()) {
-              if (!skip_mma || accf == 0) {
-                if (nmma == 4) {
-                  // K-major SW128: 8-row groups are 1024 B apart; advancing K by 8 fp32 = +32 B inside the swizzle atom
-                  mma_lohi<BF16>(tmem_d, a_lo, ahi, b_lo, bhi, idesc, accf);
-                  mma_lohi<BF16>(tmem_d, a_lo + 2, ahi, b_lo + 2, bhi, idesc, 1u);
-                  mma_lohi<BF16>(tmem_d, a_lo + 4, ahi, b_lo + 4, bhi, idesc, 1u);
-                  mma_lohi<BF16>(tmem_d, a_lo + 6, ahi, b_lo + 6, bhi, idesc, 1u);
-                } else {
-                  for (int k = 0; k < nmma; ++k)
-                    mma_lohi<BF16>(tmem_d, a_lo + 2 * k, ahi, b_lo + 2 * k, bhi, idesc, k > 0 ? 1u : accf);
-                }
-              }
-              // frees this smem stage (in every CTA that multicasts into it) once the MMAs above have read it
-              if (csize == 1) tc_commit(&ctl->empty[stage]); else tc_commit_mc(&ctl->empty[stage], cmask);
+              mbar_expect_tx(&ctl->full[stage], kABytes + b_bytes);
+              tma_load_5d(sa, &pm->tmA, &ctl->full[stage], kb * KE, cpx, cx, cpy, cy);
+              tma_load_2d(sa + kABytes, &pm->tmB, &ctl->full[stage], kb * KE, tap * n_total + n_off);
             }
             __syncwarp();
-            accf = 1u;
             if (++stage == p.stages) { stage = 0; phase ^= 1; }
           }
         }
-        if (elect_one()) {
-          tc_commit(&ctl->tmem_full[b0]);
-          if (pair) tc_commit(&ctl->tmem_full[b1]);
-        }
-        __syncwarp();
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
       }
     }
   } else if (warp >= 4) {
-    // ===================================================================== epilogue (128 threads)
-    const int ew = warp - 4;             // TMEM lane quarter = warp % 4
-    const int et = threadIdx.x - 128;    // 0..127
-    const int row = ew * 32 + lane;      // tile row (pixel) owned by this thread
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    double stat_s1 = 0.0, stat_s2 = 0.0;
-    const int bw_shift = 31 - __clz(p.bw);  // tile widths are powers of two
-    if (pair) {
-      // ------------------------------------------------------------------ pair mode (n_mma == 128, n_split == 1)
-      // Per iteration: two tiles (upper / lower) x two 64-channel halves.  A half = 2 chunks of the staging buffer: TMEM ->
-      // (+bias) -> swizzled smem -> TMA store; BN statistics of those 64 channels are taken from the staged copy by 128
-      // threads = 64 channels x 2 row halves.  A thread therefore owns two channels (one per half) of one row half.
-      double ps1[2] = {0.0, 0.0}, ps2[2] = {0.0, 0.0};
-      const int cl = et & 63, rh = et >> 6;
-      for (int it = 0; it < n_iters; ++it) {
-        const int tile = tile0 + it * tile_stride;
-        const int tx = tile % p.tiles_x, typ = tile / p.tiles_x;
-        const int x0 = tx * p.bw;
-        const int n_rounds = (p.n_chunks + 1) / 2;   // 64 channels per staging round
-        for (int sub = 0; sub < 2; ++sub) {
-          const int g = 2 * it + sub, buf = g % nbuf;
-          mbar_wait(&ctl->tmem_full[buf], (g / nbuf) & 1);
-          tc_fence_after();
-          const int y0 = (2 * typ + sub) * p.bh;
-          const uint32_t taddr = tmem_base + buf * acc_cols + (static_cast<uint32_t>(ew * 32) << 16);
-          for (int half = 0; half < n_rounds; ++half) {
-            if (et == 0) tma_store_wait_read0();   // the previous half's TMA store has finished reading the staging buffer
-            named_bar_sync(1, 128);                // (and every thread is past its statistics pass over it)
-#pragma unroll
-            for (int jj = 0; jj < 2; ++jj) {
-              const int j = half * 2 + jj;
-              if (j >= p.n_chunks) break;
-              uint32_t v[32];
-              tmem_ld_32x32(taddr + j * 32, v);
-              tmem_ld_wait();
-              uint8_t* rowp = staging + jj * kChunkBytes + row * 128;
-#pragma unroll
-              for (int q = 0; q < 8; ++q) {
-                float4 o;
-                o.x = __uint_as_float(v[q * 4 + 0]) + ctl->bias[j * 32 + q * 4 + 0];
-                o.y = __uint_as_float(v[q * 4 + 1]) + ctl->bias[j * 32 + q * 4 + 1];
-                o.z = __uint_as_float(v[q * 4 + 2]) + ctl->bias[j * 32 + q * 4 + 2];
-                o.w = __uint_as_float(v[q * 4 + 3]) + ctl->bias[j * 32 + q * 4 + 3];
-                *reinterpret_cast<float4*>(rowp + ((q ^ (row & 7)) << 4)) = o;
-              }
-            }
-            if (half == n_rounds - 1) {   // this tile's accumulator is drained -> its buffer goes back to the MMA warp
-              tc_fence_before();
-              __syncwarp();
-              if (lane == 0) mbar_arrive(&ctl->tmem_empty[buf]);
-            }
-            fence_proxy_async_smem();
-            named_bar_sync(1, 128);
-            if (et == 0) {
-              for (int jj = 0; jj < 2 && half * 2 + jj < p.n_chunks; ++jj)
-                tma_store_3d(&pm->tmD, staging + jj * kChunkBytes, (half * 2 + jj) * 32, x0, y0);
-              tma_store_commit();
-            }
-            if (p.stats != nullptr) {   // n_mma == 128 only (two rounds): the launcher rejects statistics on wider tiles
-              const int jj = cl >> 5, q = (cl & 31) >> 2, e = cl & 3;
-              const uint8_t* cb = staging + jj * kChunkBytes + e * 4;
-              float a0 = 0.f, a1 = 0.f, b0 = 0.f, b1 = 0.f;
-              const int m0 = rh * 64;
-              if (x0 + p.bw <= p.out_w && y0 + p.bh <= p.out_h) {
-#pragma unroll 8
-                for (int m = m0; m < m0 + 64; m += 2) {
-                  const float x = *reinterpret_cast<const float*>(cb + m * 128 + ((q ^ (m & 7)) << 4));
-                  const float y = *reinterpret_cast<const float*>(cb + (m + 1) * 128 + ((q ^ ((m + 1) & 7)) << 4));
-                  a0 += x; b0 = fmaf(x, x, b0);
-                  a1 += y; b1 = fmaf(y, y, b1);
-                }
-              } else {
-                for (int m = m0; m < m0 + 64; ++m) {
-                  const int py = m >> bw_shift, px = m & (p.bw - 1);
-                  if (x0 + px < p.out_w && y0 + py < p.out_h) {
-                    const float x = *reinterpret_cast<const float*>(cb + m * 128 + ((q ^ (m & 7)) << 4));
-                    a0 += x; b0 = fmaf(x, x, b0);
-                  }
-                }
-              }
-              ps1[half & 1] += static_cast<double>(a0 + a1);
-              ps2[half & 1] += static_cast<double>(b0 + b1);
-            }
-          }
-        }
-      }
-      if (p.stats != nullptr) {
-        const int rep = (blockIdx.x % kAccR) * kAccLine;
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          const int c = half * 64 + cl;
-          if (c < p.stats_ld) {
-            atomicAdd(&p.stats[c * kAccStride + rep], ps1[half]);
-            atomicAdd(&p.stats[(p.stats_ld + c) * kAccStride + rep], ps2[half]);
-          }
-        }
-      }
-    } else
-    for (int it = 0; it < n_iters; ++it) {
-      const int tile = tile0 + it * tile_stride;
-      int tx = tile % p.tiles_x, ty = tile / p.tiles_x;
-      int opx = 0, opy = 0;
-      if (p.nphase > 0) {
-        if (tile >= num_tiles) break;
-        const int t = tile % tiles_pp;
-        tx = t % p.tiles_x; ty = t / p.tiles_x;
-        opx = p.phs[tile / tiles_pp].opx; opy = p.phs[tile / tiles_pp].opy;
-      }
-      const int x0 = tx * p.bw, y0 = ty * p.bh;
-      mbar_wait(&ctl->tmem_full[acc], acc_phase);
-      tc_fence_after();
-      // staging buffer must be free (previous tile's TMA store has finished reading it)
-      if (et == 0) tma_store_wait_read0();
-      named_bar_sync(1, 128);
-      const uint32_t taddr = tmem_base + acc * acc_cols + (static_cast<uint32_t>(ew * 32) << 16);
-      if (p.dbg_flags & 4) {
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&ctl->tmem_empty[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        continue;
-      }
-      for (int j = 0; j < p.n_chunks; ++j) {
-        uint32_t v[32];
-        tmem_ld_32x32(taddr + j * 32, v);
-        tmem_ld_wait();
-        uint8_t* rowp = staging + j * kChunkBytes + row * 128;
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          float4 o;
-          o.x = __uint_as_float(v[q * 4 + 0]) + ctl->bias[j * 32 + q * 4 + 0];
-          o.y = __uint_as_float(v[q * 4 + 1]) + ctl->bias[j * 32 + q * 4 + 1];
-          o.z = __uint_as_float(v[q * 4 + 2]) + ctl->bias[j * 32 + q * 4 + 2];
-          o.w = __uint_as_float(v[q * 4 + 3]) + ctl->bias[j * 32 + q * 4 + 3];
-          *reinterpret_cast<float4*>(rowp + ((q ^ (row & 7)) << 4)) = o;  // 128B swizzle (matches the TMA map)
-        }
-      }
-      // accumulator drained -> hand TMEM buffer back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&ctl->tmem_empty[acc]);
-      fence_proxy_async_smem();
-      named_bar_sync(1, 128);
-      if (et == 0) {
-        if (p.nphase > 0)
-          for (int j = 0; j < p.n_chunks; ++j) tma_store_5d(&pm->tmD, staging + j * kChunkBytes, n_off + j * 32, opx, x0, opy, y0);
-        else
-          for (int j = 0; j < p.n_chunks; ++j) tma_store_3d(&pm->tmD, staging + j * kChunkBytes, n_off + j * 32, x0, y0);
-        tma_store_commit();
-      }
-      if (p.stats != nullptr && et < p.n_mma) {
-        // per-channel sum / sum-of-squares of this tile (feeds the following BatchNorm): thread = channel et, running
-        // totals stay in registers across all tiles of this persistent CTA (one fp64 atomic pair per thread at the end)
-        const int c = et;
-        const int j = c >> 5, q = (c & 31) >> 2, e = c & 3;
-        const uint8_t* cb = staging + j * kChunkBytes + e * 4;
-        float a0 = 0.f, a1 = 0.f, b0 = 0.f, b1 = 0.f;
-        if (x0 + p.bw <= p.out_w && y0 + p.bh <= p.out_h) {
-#pragma unroll 8
-          for (int m = 0; m < kTileM; m += 2) {
-            const float x = *reinterpret_cast<const float*>(cb + m * 128 + ((q ^ (m & 7)) << 4));
-            const float y = *reinterpret_cast<const float*>(cb + (m + 1) * 128 + ((q ^ ((m + 1) & 7)) << 4));
-            a0 += x; b0 = fmaf(x, x, b0);
-            a1 += y; b1 = fmaf(y, y, b1);
-          }
-        } else {
-          for (int m = 0; m < kTileM; ++m) {
-            const int py = m >> bw_shift, px = m & (p.bw - 1);
-            if (x0 + px < p.out_w && y0 + py < p.out_h) {
-              const float x = *reinterpret_cast<const float*>(cb + m * 128 + ((q ^ (m & 7)) << 4));
-              a0 += x; b0 = fmaf(x, x, b0);
-            }
-          }
-        }
-        stat_s1 += static_cast<double>(a0 + a1);
-        stat_s2 += static_cast<double>(b0 + b1);
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+    // ===================================================================== wgmma + epilogue (one warpgroup)
+    switch (nt) {
+      case 32: tc_conv_consumer<BF16, 32>(p, pm, ctl, stage_base, stage_bytes, staging, n_iters, tile0, tile_stride, num_tiles, tiles_pp, n_off); break;
+      case 64: tc_conv_consumer<BF16, 64>(p, pm, ctl, stage_base, stage_bytes, staging, n_iters, tile0, tile_stride, num_tiles, tiles_pp, n_off); break;
+      case 96: tc_conv_consumer<BF16, 96>(p, pm, ctl, stage_base, stage_bytes, staging, n_iters, tile0, tile_stride, num_tiles, tiles_pp, n_off); break;
+      case 128: tc_conv_consumer<BF16, 128>(p, pm, ctl, stage_base, stage_bytes, staging, n_iters, tile0, tile_stride, num_tiles, tiles_pp, n_off); break;
+      default: tc_conv_consumer<BF16, 160>(p, pm, ctl, stage_base, stage_bytes, staging, n_iters, tile0, tile_stride, num_tiles, tiles_pp, n_off); break;
     }
-    if (!pair && p.stats != nullptr && et < p.n_mma && n_off + et < p.stats_ld) {
-      const int rep = (blockIdx.x % kAccR) * kAccLine;
-      atomicAdd(&p.stats[(n_off + et) * kAccStride + rep], stat_s1);
-      atomicAdd(&p.stats[(p.stats_ld + n_off + et) * kAccStride + rep], stat_s2);
-    }
-    if (et == 0) tma_store_wait_all0();
   }
-
-  tc_fence_before();
   __syncthreads();
-  if (csize > 1) cluster_sync_all();  // no CTA may exit while a peer can still multicast into it / arrive on its barriers
-  if (!DEEP && warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, tmem_cols_pow2(nbuf * acc_cols));
-  }
 }
 __global__ void __launch_bounds__(kNumThreads, 1) tc_conv_kernel(const __grid_constant__ TcConvParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  tc_conv_body<false>(p, &p, smem_raw, 0u);
+  tc_conv_body<false>(p, &p, smem_raw);
 }
 __global__ void __launch_bounds__(kNumThreads, 1) tc_conv_kernel_bf16(const __grid_constant__ TcConvParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  tc_conv_body<false, true>(p, &p, smem_raw, 0u);
+  tc_conv_body<false, true>(p, &p, smem_raw);
 }
 
 // ------------------------------------------------------------------------------------------------ wgrad
 struct SmemCtlW {
   uint64_t full[8];
   uint64_t empty[8];
-  uint64_t tmem_full;
-  uint32_t tmem_base;
 };
 
-// BF16 = true: dY and X are bf16; a chunk is 64 channels x kp pixel rows of 128 bytes in the standard 128-byte swizzle
-// (16-byte atoms: MN-major 16-bit operands need no 32-byte-atom layout), K = 16 pixels per MMA.
+// Consumer warpgroup of the wgrad kernel, NT = accumulator columns per tap (p.n_cols).  Per pixel block: transpose the
+// pixel-major stage (dY: 128 channels, X: NT channels, kWgradKp pixels each, 128-byte swizzled rows of 32 fp32 / 64 bf16 channels)
+// into K-major swizzled tiles At [128 rows][kWgradKp pixels] and Bt [NT rows][kWgradKp pixels], then D[n][c] += At * Bt^T.
+template <bool BF16, int NT>
+__device__ __forceinline__ void tc_wgrad_consumer(const TcWgradParams& p, SmemCtlW* ctl, uint8_t* smem, int stage_bytes,
+                                                  uint8_t* tbase, int items) {
+  constexpr int KE = BF16 ? 64 : 32;                 // channels per 128-byte source row
+  constexpr int E = BF16 ? 2 : 4;                    // bytes per element
+  constexpr int kTA = kTileM * 128;                  // At: 128 rows of 128 bytes
+  constexpr int kTBuf = kTA + ((NT * 128 + 1023) & ~1023);
+  constexpr int kRows = 128 + NT;
+  const int et = threadIdx.x - 128;
+  const int w = et >> 5, lane = et & 31;
+  constexpr int chunk_bytes = kWgradKp * 128;
+  constexpr int y_bytes = (128 / KE) * chunk_bytes;
+  constexpr int groups = kWgradKp * E / 16;          // 16-byte K groups per transposed row
+  constexpr int nk = kWgradKp / (BF16 ? 16 : 8);     // wgmma K steps per pixel block
+  const int taps = p.kh * p.kw;
+  int stage = 0, tb = 0;
+  uint32_t phase = 0;
+  float acc[2][NT / 2];
+  for (int item = blockIdx.x; item < items; item += gridDim.x) {
+    const int tap = item / p.ksplits, ks = item % p.ksplits;
+    const int blk0 = static_cast<int>((static_cast<long long>(p.px_blocks) * ks) / p.ksplits);
+    const int blk1 = static_cast<int>((static_cast<long long>(p.px_blocks) * (ks + 1)) / p.ksplits);
+#pragma unroll
+    for (int i = 0; i < NT / 2; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
+    for (int blk = blk0; blk < blk1; ++blk) {
+      mbar_wait(&ctl->full[stage], phase);
+      named_bar_sync(1, 128);   // every thread is past the wait of the wgmmas that last read buffer tb
+      const uint8_t* sy = smem + stage * stage_bytes;
+      const uint8_t* sx = sy + y_bytes;
+      uint8_t* ta = tbase + tb * kTBuf;
+      uint8_t* tbb = ta + kTA;
+      for (int i = et; i < kRows * groups; i += 128) {
+        const int g = i / kRows, row = i % kRows;
+        const bool is_y = row < 128;
+        const int rs = is_y ? row : row - 128;
+        const uint8_t* src = (is_y ? sy : sx) + (rs / KE) * chunk_bytes;
+        const int cb = (rs % KE) * E;                 // byte of this channel inside a source row
+        uint32_t v[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          if (BF16) {
+            const int px = g * 8 + 2 * u;
+            const uint32_t lo = *reinterpret_cast<const uint16_t*>(src + px * 128 + ((((cb >> 4) ^ (px & 7)) << 4) | (cb & 15)));
+            const uint32_t hi = *reinterpret_cast<const uint16_t*>(src + (px + 1) * 128 + ((((cb >> 4) ^ ((px + 1) & 7)) << 4) | (cb & 15)));
+            v[u] = lo | (hi << 16);
+          } else {
+            const int px = g * 4 + u;
+            v[u] = *reinterpret_cast<const uint32_t*>(src + px * 128 + ((((cb >> 4) ^ (px & 7)) << 4) | (cb & 15)));
+          }
+        }
+        uint8_t* dst = (is_y ? ta : tbb) + rs * 128 + ((g ^ (rs & 7)) << 4);
+        *reinterpret_cast<uint4*>(dst) = make_uint4(v[0], v[1], v[2], v[3]);
+      }
+      fence_proxy_async_smem();
+      named_bar_sync(1, 128);
+      if (lane == 0) mbar_arrive(&ctl->empty[stage]);   // the stage is fully read: TMA may refill it
+      const uint32_t a_lo = desc_lo(smem_u32(ta)), b_lo = desc_lo(smem_u32(tbb));
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < nk; ++k) {
+        wgmma_ss<NT, BF16>(acc[0], desc_of(a_lo + 2 * k), desc_of(b_lo + 2 * k));
+        wgmma_ss<NT, BF16>(acc[1], desc_of(a_lo + ((64u * 128u) >> 4) + 2 * k), desc_of(b_lo + 2 * k));
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      tb ^= 1;
+      if (++stage == p.stages) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    float* dst = p.partial + (static_cast<size_t>(ks) * taps + tap) * 128 * NT;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int j = 0; j < NT / 8; ++j) {
+        const int col = 8 * j + 2 * (lane & 3);
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const int n = 64 * h + 16 * w + (lane >> 2) + 8 * rr;   // output channel
+          *reinterpret_cast<float2*>(dst + static_cast<size_t>(n) * NT + col) =
+              make_float2(acc[h][4 * j + 2 * rr], acc[h][4 * j + 2 * rr + 1]);
+        }
+      }
+    }
+  }
+}
+
 template <bool DEEP, bool BF16 = false>
-__device__ __forceinline__ void tc_wgrad_body(const TcWgradParams& p, const TcWgradParams* pm, uint8_t* smem_raw, uint32_t tmem_pre) {
-  if (DEEP && static_cast<int>(blockIdx.x) >= p.kh * p.ksplits) return;
+__device__ __forceinline__ void tc_wgrad_body(const TcWgradParams& p, const TcWgradParams* pm, uint8_t* smem_raw) {
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr int KE = BF16 ? 64 : 32;                           // channels per 128-byte row
   constexpr int YCH = 128 / KE;                                // chunks of dY (128 channels)
-  const int chunk_bytes = p.kp * 128;                          // kp pixel rows x KE channels
+  constexpr int chunk_bytes = kWgradKp * 128;                  // kWgradKp pixel rows x KE channels
   const int y_bytes = YCH * chunk_bytes;                       // dY: 128 channels
-  // X operand: per tap column its own kp-pixel tile, or (xshare: stride 1) ONE (kp + kw - 1)-pixel tile that all tap
-  // columns read through row-shifted descriptors (swizzling is a function of the absolute smem address)
-  const int xrows = p.xshare ? p.kp + p.kw - 1 : p.kp;
-  const int xchunk = p.xshare ? ((xrows * 128 + 1023) & ~1023) : chunk_bytes;
-  const int x_bytes = p.c_chunks * xchunk;                     // X : c_pad channels
-  const int stage_bytes = y_bytes + (p.xshare ? 1 : p.kw) * x_bytes;
-  const int stage_tx = y_bytes + (p.xshare ? p.c_chunks * xrows * 128 : p.kw * x_bytes);
-  SmemCtlW* ctl = reinterpret_cast<SmemCtlW*>(smem + p.stages * stage_bytes);
+  const int x_bytes = p.c_chunks * chunk_bytes;                // X : c_pad channels
+  const int stage_bytes = y_bytes + x_bytes;
+  uint8_t* tbase = smem + p.stages * stage_bytes;              // two transposed operand buffers
+  const int tbuf = kTileM * 128 + round1024(p.n_cols * 128);
+  SmemCtlW* ctl = reinterpret_cast<SmemCtlW*>(tbase + 2 * tbuf);
+  const int items = p.kh * p.kw * p.ksplits;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int r = blockIdx.x / p.ksplits;   // filter row handled by this CTA
-  const int ks = blockIdx.x % p.ksplits;  // split-K index
-  const int c_pad = p.n_cols > 0 ? p.n_cols : p.c_chunks * 32;   // UMMA N = accumulator columns per tap = row stride of the output
-  const uint32_t ncols = tmem_cols_pow2(p.kw * c_pad);
-  const int blk0 = static_cast<int>((static_cast<long long>(p.px_blocks) * ks) / p.ksplits);
-  const int blk1 = static_cast<int>((static_cast<long long>(p.px_blocks) * (ks + 1)) / p.ksplits);
-
   if (!DEEP) pdl_trigger();
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&pm->tmY);
@@ -630,164 +398,74 @@ __device__ __forceinline__ void tc_wgrad_body(const TcWgradParams& p, const TcWg
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < p.stages; ++i) {
       mbar_init(&ctl->full[i], 1);
-      mbar_init(&ctl->empty[i], 1);
+      mbar_init(&ctl->empty[i], 4);   // one arrival per consumer warp
     }
-    mbar_init(&ctl->tmem_full, 1);
     fence_mbar_init();
   }
-  if (warp == 2) {
-    if (!DEEP) {
-      tmem_alloc(&ctl->tmem_base, ncols);
-      tmem_relinquish();
-    }
-  }
   if (!DEEP) pdl_wait();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = DEEP ? tmem_pre : ctl->tmem_base;
 
   if (warp == 0) {
-    {
-      int stage = 0;
-      uint32_t phase = 0;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int item = blockIdx.x; item < items; item += gridDim.x) {
+      const int tap = item / p.ksplits, ks = item % p.ksplits;
+      const int r = tap / p.kw, s = tap % p.kw;
+      const int blk0 = static_cast<int>((static_cast<long long>(p.px_blocks) * ks) / p.ksplits);
+      const int blk1 = static_cast<int>((static_cast<long long>(p.px_blocks) * (ks + 1)) / p.ksplits);
+      const int ix = p.offx + s, iy = p.offy + r;
       for (int blk = blk0; blk < blk1; ++blk) {
         const int y = blk / p.px_blocks_x;
-        const int x0 = (blk % p.px_blocks_x) * p.kp;
+        const int x0 = (blk % p.px_blocks_x) * kWgradKp;
+        int cpx, cx, cpy, cy;
+        if (p.stride == 1) {
+          cpx = 0; cx = x0 + ix; cpy = 0; cy = y + iy;
+        } else {
+          cpx = ix & 1; cx = x0 + (ix >> 1); cpy = iy & 1; cy = y + (iy >> 1);
+        }
         mbar_wait(&ctl->empty[stage], phase ^ 1);
         uint8_t* sy = smem + stage * stage_bytes;
         if (elect_one()) {
-        mbar_expect_tx(&ctl->full[stage], stage_tx);
-        for (int j = 0; j < YCH; ++j) tma_load_3d(sy + j * chunk_bytes, &pm->tmY, &ctl->full[stage], j * KE, x0, y);
-        if (p.xshare) {
-          uint8_t* sx = sy + y_bytes;
+          mbar_expect_tx(&ctl->full[stage], stage_bytes);
+          for (int j = 0; j < YCH; ++j) tma_load_3d(sy + j * chunk_bytes, &pm->tmY, &ctl->full[stage], j * KE, x0, y);
           for (int j = 0; j < p.c_chunks; ++j)
-            tma_load_5d(sx + j * xchunk, &pm->tmX, &ctl->full[stage], j * KE, 0, x0 + p.offx, 0, y + p.offy + r);
-        } else
-        for (int s = 0; s < p.kw; ++s) {
-          const int ix = p.offx + s, iy = p.offy + r;
-          int cpx, cx, cpy, cy;
-          if (p.stride == 1) {
-            cpx = 0; cx = x0 + ix; cpy = 0; cy = y + iy;
-          } else {
-            cpx = ix & 1; cx = x0 + (ix >> 1); cpy = iy & 1; cy = y + (iy >> 1);
-          }
-          uint8_t* sx = sy + y_bytes + s * x_bytes;
-          for (int j = 0; j < p.c_chunks; ++j)
-            tma_load_5d(sx + j * chunk_bytes, &pm->tmX, &ctl->full[stage], j * KE, cpx, cx, cpy, cy);
-        }
+            tma_load_5d(sy + y_bytes + j * chunk_bytes, &pm->tmX, &ctl->full[stage], j * KE, cpx, cx, cpy, cy);
         }
         __syncwarp();
         if (++stage == p.stages) { stage = 0; phase ^= 1; }
       }
-    }
-  } else if (warp == 1) {
-    {
-      // A = dY (M = 128 output channels), B = X (N = c_pad input channels); both MN-major, K = pixels.
-      const uint32_t idesc = BF16 ? make_idesc_bf16(128, c_pad, 1, 1) : make_idesc_tf32(128, c_pad, 1, 1);
-      // MN-major tf32 must use the 32-byte-atom 128B swizzle: 32-channel chunks are LBO = chunk_bytes apart,
-      // 4-pixel K atoms are SBO = 512 B apart; one K=8 MMA consumes 8 pixel rows = 1024 B (lo += 64).
-      // bf16: standard 128B swizzle, 8-pixel K groups SBO = 1024 B apart, one K=16 MMA consumes 16 pixel rows = 2048 B
-      const uint32_t hi = BF16 ? desc_hi(1024, 2) : desc_hi(512, 1);
-      constexpr uint32_t kstep = BF16 ? 128u : 64u;
-      const uint32_t y_lo0 = desc_lo(smem_u32(smem), chunk_bytes);
-      const uint32_t stage_step = static_cast<uint32_t>(stage_bytes) >> 4;
-      // X descriptor: LBO = its own chunk stride; per tap column either the next tile or +1 pixel row (128 B)
-      const uint32_t x_off = ((static_cast<uint32_t>(y_bytes) >> 4) + ((static_cast<uint32_t>(xchunk) >> 4) << 16)) -
-                             ((static_cast<uint32_t>(chunk_bytes) >> 4) << 16);
-      const uint32_t x_step = p.xshare ? 8u : (static_cast<uint32_t>(x_bytes) >> 4);
-      const int nk = p.kp / (BF16 ? 16 : 8);
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t accf = 0;
-      for (int blk = blk0; blk < blk1; ++blk) {
-        mbar_wait(&ctl->full[stage], phase);
-        tc_fence_after();
-        const uint32_t y_lo = y_lo0 + stage * stage_step;
-        if (elect_one()) {
-          uint32_t x_lo = y_lo + x_off;
-          uint32_t td = tmem_base;
-          for (int s = 0; s < p.kw; ++s) {
-            mma_lohi<BF16>(td, y_lo, hi, x_lo, hi, idesc, accf);
-            for (int k = 1; k < nk; ++k) mma_lohi<BF16>(td, y_lo + kstep * k, hi, x_lo + kstep * k, hi, idesc, 1u);
-            x_lo += x_step;
-            td += c_pad;
-          }
-          tc_commit(&ctl->empty[stage]);
-        }
-        __syncwarp();
-        accf = 1u;
-        if (++stage == p.stages) { stage = 0; phase ^= 1; }
-      }
-      if (elect_one()) tc_commit(&ctl->tmem_full);
-      __syncwarp();
     }
   } else if (warp >= 4) {
-    const int ew = warp - 4;
-    const int n = ew * 32 + lane;  // output channel (TMEM lane)
-    if (blk1 > blk0) {
-      mbar_wait(&ctl->tmem_full, 0);
-      tc_fence_after();
-    }
-    for (int s = 0; s < p.kw; ++s) {
-      if (p.atomic && blk1 <= blk0) break;   // nothing accumulated by this CTA
-      const int tap = r * p.kw + s;
-      float* dst = p.partial + ((static_cast<size_t>(p.atomic ? 0 : ks) * (p.kh * p.kw) + tap) * 128 + n) * c_pad;
-      for (int j = 0; j < c_pad / 32; ++j) {
-        uint32_t v[32];
-        if (blk1 > blk0) {
-          tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + s * c_pad + j * 32, v);
-          tmem_ld_wait();
-        } else {
-#pragma unroll
-          for (int q = 0; q < 32; ++q) v[q] = 0u;
-        }
-        if (p.atomic) {
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            red_add_v4(dst + j * 32 + q * 4, __uint_as_float(v[q * 4]), __uint_as_float(v[q * 4 + 1]),
-                       __uint_as_float(v[q * 4 + 2]), __uint_as_float(v[q * 4 + 3]));
-          continue;
-        }
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          float4 o = make_float4(__uint_as_float(v[q * 4]), __uint_as_float(v[q * 4 + 1]),
-                                 __uint_as_float(v[q * 4 + 2]), __uint_as_float(v[q * 4 + 3]));
-          *reinterpret_cast<float4*>(dst + j * 32 + q * 4) = o;
-        }
-      }
+    switch (p.n_cols) {
+      case 32: tc_wgrad_consumer<BF16, 32>(p, ctl, smem, stage_bytes, tbase, items); break;
+      case 64: tc_wgrad_consumer<BF16, 64>(p, ctl, smem, stage_bytes, tbase, items); break;
+      case 96: tc_wgrad_consumer<BF16, 96>(p, ctl, smem, stage_bytes, tbase, items); break;
+      case 128: tc_wgrad_consumer<BF16, 128>(p, ctl, smem, stage_bytes, tbase, items); break;
+      default: tc_wgrad_consumer<BF16, 160>(p, ctl, smem, stage_bytes, tbase, items); break;
     }
   }
-  tc_fence_before();
   __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    if (!DEEP) tmem_dealloc(tmem_base, ncols);
-  }
 }
 __global__ void __launch_bounds__(kNumThreads, 1) tc_wgrad_kernel(const __grid_constant__ TcWgradParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  tc_wgrad_body<false>(p, &p, smem_raw, 0u);
+  tc_wgrad_body<false>(p, &p, smem_raw);
 }
 __global__ void __launch_bounds__(kNumThreads, 1) tc_wgrad_kernel_bf16(const __grid_constant__ TcWgradParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  tc_wgrad_body<false, true>(p, &p, smem_raw, 0u);
+  tc_wgrad_body<false, true>(p, &p, smem_raw);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
 static constexpr size_t kMaxSmem = 232448;  // 227 KB
 
 size_t tc_conv_smem_bytes(const TcConvParams& p) {
-  const size_t b_bytes = (static_cast<size_t>(p.n_mma) * 128 + 1023) & ~size_t(1023);
-  const size_t patch = p.patch ? ((static_cast<size_t>(p.pw) * p.ph * 128 + 127) & ~size_t(127)) : 0;
-  const size_t tps = p.patch ? (p.tps < 1 ? 1 : p.tps) : 1;
-  return 1024 + 2 * patch + p.stages * ((p.patch ? 0 : kABytes) + tps * b_bytes) +
-         static_cast<size_t>(p.pair ? 2 : p.n_chunks) * kChunkBytes + sizeof(SmemCtl);
+  const size_t b_bytes = round1024(round32(p.n_mma) * 128);
+  return 1024 + p.stages * (kABytes + b_bytes) + static_cast<size_t>(p.n_chunks) * kChunkBytes + sizeof(SmemCtl);
 }
 size_t tc_wgrad_smem_bytes(const TcWgradParams& p) {
-  const size_t chunk = static_cast<size_t>(p.kp) * 128;
-  const size_t xchunk = p.xshare ? ((static_cast<size_t>(p.kp + p.kw - 1) * 128 + 1023) & ~size_t(1023)) : chunk;
-  return 1024 + p.stages * ((p.bf16 ? 2 : 4) * chunk + static_cast<size_t>(p.xshare ? 1 : p.kw) * p.c_chunks * xchunk) + sizeof(SmemCtlW);
+  const size_t chunk = static_cast<size_t>(kWgradKp) * 128;
+  const size_t tbuf = kTileM * 128 + round1024(p.n_cols * 128);
+  return 1024 + p.stages * ((p.bf16 ? 2 : 4) * chunk + static_cast<size_t>(p.c_chunks) * chunk) + 2 * tbuf + sizeof(SmemCtlW);
 }
 
 cudaError_t tc_kernels_init() {
@@ -800,34 +478,37 @@ cudaError_t tc_kernels_init() {
   return cudaFuncSetAttribute(tc_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxSmem);
 }
 
+static bool conv_params_ok(const TcConvParams& p) {
+  return p.n_mma >= 1 && p.n_mma <= 160 && p.n_chunks == (p.n_mma + 31) / 32 && p.stages >= 1 && p.stages <= 8 &&
+         p.kblocks >= 1 && p.nphase >= 0 && p.nphase <= 4 &&
+         (p.bw & (p.bw - 1)) == 0 && p.bw * p.bh == kTileM;
+}
+
 cudaError_t tc_conv_launch(const TcConvParams& p, int num_sms, cudaStream_t s) {
-  const int tiles = p.pair ? p.tiles_x * ((p.tiles_y + 1) / 2) : p.tiles_x * p.tiles_y * (p.nphase > 0 ? p.nphase : 1);
-  const int cs = p.csize < 1 ? 1 : p.csize;
-  if (p.nphase > 0 && (p.patch || cs != 1 || p.nphase > 4)) return cudaErrorInvalidValue;
-  if (p.pair && (!p.patch || cs != 1 || p.n_split > 1 || p.n_mma > 160 || (p.n_mma != 128 && p.stats != nullptr)))
-    return cudaErrorInvalidValue;
-  int grid = (tiles + cs - 1) / cs * cs;
-  const int cap = num_sms / cs * cs;
-  if (grid > cap) grid = cap;
+  if (!conv_params_ok(p)) return cudaErrorInvalidValue;
+  const int tiles = p.tiles_x * p.tiles_y * (p.nphase > 0 ? p.nphase : 1);
+  int grid = tiles < num_sms ? tiles : num_sms;
   if (p.n_split > 1) {
-    if (cs != 1 || tiles * p.n_split > num_sms) return cudaErrorInvalidValue;
+    if (tiles * p.n_split > num_sms) return cudaErrorInvalidValue;
     grid = tiles * p.n_split;   // one CTA per (tile, channel part)
   }
   const size_t smem = tc_conv_smem_bytes(p);
   if (smem > kMaxSmem) return cudaErrorInvalidValue;
-  return launch_k(p.bf16 ? tc_conv_kernel_bf16 : tc_conv_kernel, dim3(grid), dim3(kNumThreads), smem, s, cs, p);
+  return launch_k(p.bf16 ? tc_conv_kernel_bf16 : tc_conv_kernel, dim3(grid), dim3(kNumThreads), smem, s, 1, p);
 }
 // grid the stand-alone launch uses (the persistent deep-level kernel runs the same CTA -> tile mapping on its first vgrid CTAs)
 int tc_conv_grid(const TcConvParams& p, int num_sms) {
-  const int tiles = p.pair ? p.tiles_x * ((p.tiles_y + 1) / 2) : p.tiles_x * p.tiles_y * (p.nphase > 0 ? p.nphase : 1);
+  const int tiles = p.tiles_x * p.tiles_y * (p.nphase > 0 ? p.nphase : 1);
   if (p.n_split > 1) return tiles * p.n_split;
   return tiles < num_sms ? tiles : num_sms;
 }
 
 cudaError_t tc_wgrad_launch(const TcWgradParams& p, cudaStream_t s) {
   const size_t smem = tc_wgrad_smem_bytes(p);
-  if (smem > kMaxSmem) return cudaErrorInvalidValue;
-  return launch_k(p.bf16 ? tc_wgrad_kernel_bf16 : tc_wgrad_kernel, dim3(p.kh * p.ksplits), dim3(kNumThreads), smem, s, 1, p);
+  if (smem > kMaxSmem || p.n_cols % 32 != 0 || p.n_cols < 32 || p.n_cols > 160 ||
+      p.stages < 1 || p.stages > 8)
+    return cudaErrorInvalidValue;
+  return launch_k(p.bf16 ? tc_wgrad_kernel_bf16 : tc_wgrad_kernel, dim3(p.kh * p.kw * p.ksplits), dim3(kNumThreads), smem, s, 1, p);
 }
 
 }  // namespace dip

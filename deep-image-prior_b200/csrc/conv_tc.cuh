@@ -1,4 +1,4 @@
-// Host-side descriptors for the tcgen05 implicit-GEMM convolution kernels (conv_tc.cu).
+// Host-side descriptors for the wgmma implicit-GEMM convolution kernels (conv_tc.cu).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -21,19 +21,12 @@ struct TcConvParams {
   int kh, kw;              // filter taps
   int stride;              // 1 or 2 (spatial stride of A reads)
   int offx, offy;          // input coordinate of tap (0,0) for output pixel (0,0)
-  int bf16;                // 1: bf16 operands (kind::f16): A / Wp are bf16, a K block is 64 channels (still 128 bytes), K = 16 per MMA
+  int bf16;                // 1: bf16 operands: A / Wp are bf16, a K block is 64 channels (still 128 bytes), K = 16 per wgmma
   int kblocks;             // K blocks (128-byte operand rows: 32 fp32 or 64 bf16 channels) per tap
-  int tail_mmas;           // number of MMAs (K = 8 fp32 / 16 bf16 channels) issued for the last K block of a tap (1..4)
-  int n_mma;               // UMMA N of this CTA (multiple of 16, <= 160): all output channels, or N / n_split of them
+  int n_mma;               // output channels of this CTA (multiple of 16, <= 160): all of them, or N / n_split; the wgmma N is
+                           // n_mma rounded up to 32 (columns past n_mma are never stored or counted)
   int n_chunks;            // output 32-channel chunks written (ceil(n_mma/32))
   int stages;              // smem pipeline depth
-  int patch;               // 1: 3x3 stride-1 patch mode (tile 8 x 16; one (bw+2) x (bh+2) input patch serves all taps)
-  int pw, ph;              // patch extent in pixels
-  int tps;                 // patch mode: filter taps per weight stage (1..3; 3 = one filter row per barrier round)
-  int csize;               // thread-block cluster size (1, 2, 4): the weight tile is multicast across the cluster
-  int pair;                // patch mode, n_mma == 128: every CTA iteration computes TWO vertically adjacent tiles from one
-                           // (bw+2) x (2*bh+2) input patch and ONE stream of weight tiles (two accumulators per TMEM buffer):
-                           // half the L2->SM weight traffic and half the barrier rounds per FLOP
   int n_split;             // 1, 2 or 4 CTAs per pixel tile, each computing n_mma = N / n_split output channels (small levels)
   // Stride-2 input gradient as its 4 sub-pixel phases in ONE launch (nphase = 4, per-tap mode): output pixel (2i+a, 2j+b)
   // of the padded input gradient only receives the taps r = a (mod 2), s = b (mod 2), i.e. a (2-a) x (2-b) stride-1
@@ -47,32 +40,28 @@ struct TcConvParams {
   const float* bias;       // [n_valid] or nullptr
   double* stats;           // [2][stats_ld] per-channel sum / sum of squares (fp64 atomics) or nullptr
   int stats_ld;
-  int dbg_shift;           // experiment: start the A descriptor `dbg_shift` 128-byte rows into the stage
-  int dbg_flags;           // experiments: 1 skip A loads, 2 skip B loads, 4 skip epilogue, 8 skip MMAs
-  int dbg_nmma;            // experiment: MMAs issued per k-block (patch mode)
-  int dbg_bo;              // experiment: set the descriptor's base_offset field to ((addr >> 7) & 7)
 };
 
 // Weight-gradient GEMM:  dW[tap][n][c] = sum_{pixels} dY[pixel][n] * X[pixel (+) tap][c]
 //   dY : NHWC [H][W][N] (fp32 or bf16 twin; N <= 128 output channels, channels >= N read as zero) through a 3-D map (N, W, H)
 //   X  : conv input through the same 5-D view as in TcConvParams
-//   out: atomic = 1 (engine): every split-K CTA adds its tile into ONE fp32 accumulator [tap][128][c_pad] with vector
-//        reductions at the L2 (red.global.add.v4.f32; the 0.6 MB accumulator never leaves the L2) -- no partials in
-//        HBM, no reduction kernel;  atomic = 0: deterministic partials [ksplit][tap][128][c_pad] + follow-up reduce
+//   A work item is one filter tap and one split-K range of pixel blocks (kh * kw * ksplits items); it writes its own
+//   slice of partials [ksplit][tap][128][c_pad], which a follow-up kernel sums in a fixed order -- the gradient does not
+//   depend on the order in which work items finish (fp32 atomics here made runs drift apart over thousands of steps).
+// pixels per K block of the weight-gradient GEMM (TMA box width; one transposed 128-byte row holds 32 fp32 pixels).  A row
+// shorter than a multiple of 32 reads zero-filled dY past its end, which adds nothing.
+static constexpr int kWgradKp = 32;
 struct TcWgradParams {
   CUtensorMap tmY;
   CUtensorMap tmX;
-  float* partial;          // atomic: [kh*kw][128][c_pad] accumulator (zeroed by the caller); else [ksplits][kh*kw][128][c_pad]
-  int atomic;
+  float* partial;          // [ksplits][kh*kw][128][c_pad], every element written by the kernel
   int kh, kw, stride, offx, offy;
-  int px_blocks_x;         // W / kp
+  int px_blocks_x;         // ceil(W / kWgradKp)
   int px_blocks;           // total pixel blocks = H * px_blocks_x
-  int kp;                  // pixels per K block (box width): 16 or 32
-  int bf16;                // 1: dY / X are bf16 (chunks of 64 channels, standard 128B swizzle, K = 16 pixels per MMA)
+  int bf16;                // 1: dY / X are bf16 (chunks of 64 channels, K = 16 pixels per wgmma)
   int c_chunks;            // 128-byte channel chunks of X (32 fp32 / 64 bf16 channels each)
-  int n_cols;              // UMMA N = accumulator columns per tap = row stride of `partial` (0: 32 * c_chunks)
-  int xshare;              // 1: stride-1 taps of a filter row share one (kp + kw - 1)-pixel X tile
-  int ksplits;             // CTAs per tap row
+  int n_cols;              // wgmma N = accumulator columns per tap = row stride of `partial` (multiple of 32, <= 160)
+  int ksplits;             // work items per filter tap
   int stages;
 };
 

@@ -44,16 +44,6 @@ __global__ void __launch_bounds__(256, 1) k_deep(const DeepOp* __restrict__ ops,
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   __shared__ __align__(16) TcConvParams s_conv;
   __shared__ __align__(16) TcWgradParams s_wg;
-  __shared__ uint32_t s_tmem;
-  const int warp = threadIdx.x >> 5;
-  if (warp == 2) {   // the whole TMEM, once, for every conv phase of this launch
-    tmem_alloc(&s_tmem, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = s_tmem;
   unsigned epoch = 0;
   for (int i = 0; i < nops; ++i) {
     const DeepOp* op = ops + i;
@@ -61,11 +51,11 @@ __global__ void __launch_bounds__(256, 1) k_deep(const DeepOp* __restrict__ ops,
     switch (type) {
       case DO_CONV:
         copy_to_smem(&s_conv, &op->u.conv);
-        tc_conv_body<true>(s_conv, &op->u.conv, smem_raw, tmem);
+        tc_conv_body<true>(s_conv, &op->u.conv, smem_raw);
         break;
       case DO_WGRAD:
         copy_to_smem(&s_wg, &op->u.wg);
-        tc_wgrad_body<true>(s_wg, &op->u.wg, smem_raw, tmem);
+        tc_wgrad_body<true>(s_wg, &op->u.wg, smem_raw);
         break;
       case DO_SKINNY_FWD: {
         const DeepSkinnyFwd a = op->u.skf;
@@ -112,12 +102,6 @@ __global__ void __launch_bounds__(256, 1) k_deep(const DeepOp* __restrict__ ops,
       default: break;
     }
     if (op->sync) grid_sync(bar, epoch); else __syncthreads();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 512);
   }
 }
 

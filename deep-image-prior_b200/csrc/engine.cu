@@ -1,4 +1,4 @@
-// dip-b200 engine: plan builder (shapes -> HBM buffers, TMA tensor maps, kernel schedule) and the C ABI of
+// dip engine: plan builder (shapes -> HBM buffers, TMA tensor maps, kernel schedule) and the C ABI of
 // libdip.so (include/dip.h).  Replaces the execution of the reference's skip network
 // (models/skip.py:41-100, module tree interpreted by torch.nn.Sequential) + autograd backward + Adam.
 #include <cuda.h>
@@ -48,11 +48,12 @@ static unsigned long long g_inited_mask = 0;   // one bit per device: function a
 static int engine_init() {
   int dev = 0;
   DIP_CUDA(cudaGetDevice(&dev));
-  if (dev >= 64) return fail("dip-b200: device ordinal >= 64 not supported");
+  if (dev >= 64) return fail("dip: device ordinal >= 64 not supported");
   if (g_inited_mask & (1ull << dev)) return 0;
   cudaDeviceProp prop;
   DIP_CUDA(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 10) return fail("dip-b200 requires an sm_100 (B200) device; found sm_" + std::to_string(prop.major * 10 + prop.minor));
+  if (prop.major != 9 || prop.minor != 0)
+    return fail("dip requires an sm_90 (H100) device; found sm_" + std::to_string(prop.major * 10 + prop.minor));
   g_num_sms = prop.multiProcessorCount;
   void* fn = nullptr;
   cudaDriverEntryPointQueryResult q;
@@ -69,10 +70,10 @@ static int engine_init() {
 static bool is_tc(int prec) { return prec == DIP_PRECISION_TF32 || prec == DIP_PRECISION_BF16; }   // tensor-core paths
 
 static int encode_map(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_b,
-                      const cuuint32_t* box, bool atom32 = false, bool bf16 = false) {
+                      const cuuint32_t* box, bool bf16 = false) {
   cuuint32_t estr[5] = {1, 1, 1, 1, 1};
   CUresult r = g_encode(m, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, rank, const_cast<void*>(base), dims, strides_b, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, atom32 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
+                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -87,7 +88,7 @@ static int encode_map(CUtensorMap* m, const void* base, int rank, const cuuint64
 // activation [rows][cols][ld] (c valid channels) as the 5-D view (C, px, X, py, Y) used by the conv kernels
 // bf16 = true: the tensor holds bf16 (ld in elements); a box row is still 128 bytes = 64 channels
 static int map_act5(CUtensorMap* m, const void* base, int rows, int cols, int ld, int c, int stride, int bw, int bh,
-                    bool atom32 = false, bool bf16 = false) {
+                    bool bf16 = false) {
   const cuuint64_t e = bf16 ? 2 : sizeof(float);
   cuuint64_t dims[5], str[4];
   if (stride == 1) {
@@ -98,22 +99,21 @@ static int map_act5(CUtensorMap* m, const void* base, int rows, int cols, int ld
     str[0] = ld * e; str[1] = 2 * ld * e; str[2] = (cuuint64_t)cols * ld * e; str[3] = 2 * (cuuint64_t)cols * ld * e;
   }
   cuuint32_t box[5] = {bf16 ? 64u : 32u, 1, (cuuint32_t)bw, 1, (cuuint32_t)bh};
-  return encode_map(m, base, 5, dims, str, box, atom32, bf16);
+  return encode_map(m, base, 5, dims, str, box, bf16);
 }
-static int map_act3(CUtensorMap* m, const void* base, int rows, int cols, int ld, int c, int bw, int bh, bool atom32 = false,
-                    bool bf16 = false) {
+static int map_act3(CUtensorMap* m, const void* base, int rows, int cols, int ld, int c, int bw, int bh, bool bf16 = false) {
   const cuuint64_t e = bf16 ? 2 : sizeof(float);
   cuuint64_t dims[3] = {(cuuint64_t)c, (cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t str[2] = {ld * e, (cuuint64_t)cols * ld * e};
   cuuint32_t box[3] = {bf16 ? 64u : 32u, (cuuint32_t)bw, (cuuint32_t)bh};
-  return encode_map(m, base, 3, dims, str, box, atom32, bf16);
+  return encode_map(m, base, 3, dims, str, box, bf16);
 }
 static int map_w2(CUtensorMap* m, const void* base, int rows_total, int kcols, int box_rows, bool bf16 = false) {
   const cuuint64_t e = bf16 ? 2 : sizeof(float);
   cuuint64_t dims[2] = {(cuuint64_t)kcols, (cuuint64_t)rows_total};
   cuuint64_t str[1] = {kcols * e};
   cuuint32_t box[2] = {bf16 ? 64u : 32u, (cuuint32_t)box_rows};
-  return encode_map(m, base, 2, dims, str, box, false, bf16);
+  return encode_map(m, base, 2, dims, str, box, bf16);
 }
 
 static void pick_tile(int w, int h, int* bw, int* bh) {
@@ -128,16 +128,6 @@ static void pick_tile(int w, int h, int* bw, int* bh) {
   }
 }
 static int round_up(int x, int m) { return (x + m - 1) / m * m; }
-// cluster size for the weight multicast: only when there is at least a full wave of tiles; the weight-tile slice of each
-// CTA must be a whole number of 8-row swizzle atoms
-static int pick_csize(int tiles, int n_rows) {
-  int want = 1;  // measured: multicast does not pay at cluster sizes <= 4 (per-SM ingest, not L2 reads, is the limit)
-  if (const char* e = getenv("DIP_CSIZE")) want = atoi(e);
-  if (tiles < 2 * 148) return 1;
-  while (want > 1 && (n_rows % (8 * want) != 0)) want >>= 1;
-  return want < 1 ? 1 : want;
-}
-
 // ------------------------------------------------------------------------------------------------ kernel timing
 // Optional CUDA-event brackets around every tensor-core launch (bench.py roofline: algorithmic FLOPs / device time).
 struct Timer {
@@ -173,54 +163,35 @@ enum HbmId { H_INPUT_PAD = 0, H_NOISE, H_SKINNY_FWD, H_BN_ACT_WRITE, H_BN_ACT_HE
   } while (0)
 
 // ------------------------------------------------------------------------------------------------ conv op
-// Filter taps per weight stage of the patch-mode convs: a barrier round costs the MMA-issuing thread a fixed ~0.2 us, so a
-// whole filter row (3 taps = 12 MMAs) per round when the stages fit, else 2 (env DIP_TPS overrides).
-static int pick_tps() {
-  if (const char* e = getenv("DIP_TPS")) { const int t = atoi(e); if (t >= 1 && t <= 3) return t; }
-  return 3;
-}
 // CTAs per pixel tile (output channels split across them) for launches with fewer tiles than SMs: n_rows % (32 * split) == 0
 static int pick_nsplit(int tiles, int n_rows) {
   int mx = 4;
   if (const char* e = getenv("DIP_NSPLIT_MAX")) mx = atoi(e);
   int sp = 1;
-  while (sp * 2 <= mx && tiles * sp * 2 <= 148 && n_rows % (32 * sp * 2) == 0) sp *= 2;
+  while (sp * 2 <= mx && tiles * sp * 2 <= g_num_sms && n_rows % (32 * sp * 2) == 0) sp *= 2;
   return sp;
 }
-// Tile pairs (TcConvParams::pair): 128 output channels (4 accumulators of 128 TMEM columns) or 144 (3 of 160), and only when
-// the wave quantisation does not eat the gain: a pair iteration costs ~1.6 single-tile iterations (measured on the level-0
-// 3x3 conv: 184.8 -> 145.9 us), so pair when ceil(pairs / SMs) * 1.6 < ceil(tiles / SMs)   (tiles_y = rows of 8 x 16 tiles)
-static int pick_pair(int tiles_x, int tiles_y, int n_rows) {
-  static const bool off = getenv("DIP_NO_PAIR") != nullptr;
-  if (off || (n_rows != 128 && n_rows != 144)) return 0;   // 144: the 132-channel dgrad (three rotating accumulators, no statistics)
-  const int sms = g_num_sms > 0 ? g_num_sms : 148;
-  const int tiles = tiles_x * tiles_y, pairs = tiles_x * ((tiles_y + 1) / 2);
-  return ((pairs + sms - 1) / sms) * 16 < ((tiles + sms - 1) / sms) * 10 ? 1 : 0;
-}
 static void fit_stages(TcConvParams& p, size_t budget = 232448) {
-  for (;;) {
-    p.stages = 6;
-    while (tc_conv_smem_bytes(p) > budget && p.stages > 2) p.stages--;
-    if (tc_conv_smem_bytes(p) <= budget || p.tps <= 1) return;
-    p.tps--;  // two stages of 3 taps do not fit (wide dgrad tiles): fall back to 2 taps per stage
-  }
+  p.stages = 6;
+  while (tc_conv_smem_bytes(p) > budget && p.stages > 2) p.stages--;
 }
 struct ConvOp {
   Timer* timer = nullptr;
   double alg_flops() const { return 2.0 * out_h * out_w * (double)N * C * k * k; }
   // N output channels (a multiple of 8, <= 128: num_channels_down / num_channels_up of the level), C input channels
   int N = 128, C = 0, k = 1, stride = 1, rot = 0;
-  int Np = 128;      // fprop UMMA N: N rounded up to 16 (rows per tap of the fprop pack; rows >= N are zero)
+  int Np = 128;      // fprop GEMM N: N rounded up to 16 (rows per tap of the fprop pack; rows >= N are zero)
   int n_pad = 128;   // dgrad K extent per tap: N rounded up to 32 (columns of the dgrad pack), n_pad16: to 64 (bf16)
   int n_pad16 = 128;
   // An op may cover a SLICE [coff, coff + C) of the (engine-order) input channels of a wider convolution whose weight has
   // Ctot input channels (the 256-channel up conv of the skip=128 configuration: fprop runs as one op with 8 K blocks,
-  // dgrad / wgrad as two 128-channel halves -- TMEM holds 512 accumulator columns).  Ctot == 0: the op is the whole conv.
+  // dgrad / wgrad as two 128-channel halves -- the register accumulators hold at most 160 columns).  Ctot == 0: the op is
+  // the whole conv.
   int Ctot = 0, coff = 0;
   bool do_fprop = true, do_wgrad = true;
   int dg_ld = 0;   // channel stride of dg_out (0: C)
   int c_pad = 0;   // fprop K extent per tap (multiple of 32)
-  int crows = 0;   // dgrad UMMA N (input channels rounded to 16)
+  int crows = 0;   // dgrad GEMM N (input channels rounded to 16)
   // precision mode bf16: the tensor-core kernels read bf16 twins of the conv input / of dY (written by the producer kernels
   // next to -- or instead of -- the fp32 tensors) and bf16 weight packs; outputs and accumulators stay fp32
   bool bf16 = false;
@@ -233,7 +204,7 @@ struct ConvOp {
   float* out = nullptr; int out_h = 0, out_w = 0;
   double* stats = nullptr;
   float* wp_f = nullptr; float* wp_d = nullptr;
-  float* wacc = nullptr;   // plan-owned weight-gradient accumulator [tap][128][c_pad] (tensor-core path; zeroed once per backward)
+  float* wacc = nullptr;   // plan-owned weight-gradient partials [ksplits][tap][128][c_pad] (tensor-core path)
   // dgrad: dg_in [dg_in_h][dg_in_w][128] -> dg_out [dg_out_h][dg_out_w][C]
   bool has_dgrad = false;
   bool dg_s2 = false;   // tensor-core dgrad of a stride-2 3x3 conv as its 4 sub-pixel phases (dg_in = dY [h][w][128], not zero-stuffed)
@@ -257,30 +228,18 @@ struct ConvOp {
   }
   size_t wp_f_elems() const { return (size_t)k * k * Np * c_pad; }
   size_t wp_d_elems() const { return (size_t)k * k * crows * n_pad; }
-  size_t wacc_elems() const { return (size_t)k * k * 128 * c_pad; }
-  // pixels per K block of the weight-gradient GEMM (TMA box width): 64 where the row length allows it -- half the barrier
-  // rounds per FLOP (bf16: 12 MMAs per round instead of 6; tf32: 24 instead of 12).  Measured (profiles/r02_wgrad_kp_ab.txt):
-  // 512^2 denoise 376.6 -> 377.7 it/s, SR 1024^2 122.0 -> 122.6 (tf32) / 150.2 -> 150.7 (bf16).  DIP_WGRAD_KP=32|64: A/B switch.
-  int wg_kp() const {
-    static const int forced = getenv("DIP_WGRAD_KP") ? atoi(getenv("DIP_WGRAD_KP")) : 0;
-    const bool want64 = forced ? forced == 64 : true;
-    return (want64 && wg_w % 64 == 0) ? 64 : (wg_w % 32 == 0) ? 32 : 16;
-  }
+  size_t wacc_elems() const { return (size_t)tc_ksplits() * k * k * 128 * c_pad; }
+  // work items per filter tap: about one item per SM of an H100 SXM over all taps (every item writes a [128][c_pad] partial
+  // slice, so more items than SMs only add traffic).  A constant, not the device's count: the plan's size is known
+  // without a device, and the split -- hence the summation order of the gradient -- is the same on every device.
   int tc_ksplits() const {
-    const int kp = wg_kp();
-    const int blocks = wg_h * ((wg_w + kp - 1) / kp);
-    int ks = 148 / k;
-    if (const char* e = getenv("DIP_WGRAD_KS")) { const int cap = atoi(e); if (cap >= 1 && cap < ks) ks = cap; }   // experiment
-    // every split-K CTA adds a whole [3 taps][128][c_pad] slab to the accumulator with L2 reductions: at the deep levels a CTA
-    // with one or two pixel blocks costs more in reductions than in MMAs, so a CTA gets at least `minblk` pixel blocks
-    static const int minblk = getenv("DIP_WGRAD_MINBLK") ? atoi(getenv("DIP_WGRAD_MINBLK")) : 1;
-    if (minblk > 1 && ks > blocks / minblk) ks = blocks / minblk;
+    const int blocks = wg_h * ((wg_w + kWgradKp - 1) / kWgradKp);
+    int ks = static_cast<int>(kNumSms) / (k * k);
     if (ks > blocks) ks = blocks;
     return ks < 1 ? 1 : ks;
   }
   size_t partial_elems(int prec) const {
-    const int ks = is_tc(prec) ? 1 : simt_ksplits;   // tensor-core path: one accumulator (atomic split-K)
-    return (size_t)ks * k * k * 128 * c_pad;
+    return is_tc(prec) ? wacc_elems() : (size_t)simt_ksplits * k * k * 128 * c_pad;
   }
 
   int build_tc(float* partial) {
@@ -288,32 +247,17 @@ struct ConvOp {
     int bw, bh;
     pick_tile(out_w, out_h, &bw, &bh);
     fp = TcConvParams{};
-    const bool patch_ok = getenv("DIP_NO_PATCH") == nullptr;
-    if (!do_fprop) {
-    } else if (k == 3 && stride == 1 && patch_ok) {
-      // patch mode: tile 8 wide x 16 tall, one 10 x 18 input patch per 32-channel block feeds all nine taps
-      bw = 8; bh = 16;
-      fp.patch = 1; fp.pw = bw + 2; fp.ph = bh + 2;
-      fp.pair = pick_pair((out_w + bw - 1) / bw, (out_h + bh - 1) / bh, Np);
-      if (fp.pair) fp.ph = 2 * bh + 2;
-      DIP_CHECK(bf16 ? map_act5(&fp.tmA, in16, in_rows, in_cols, in_ld16, C, 1, fp.pw, fp.ph, false, true)
-                     : map_act5(&fp.tmA, in, in_rows, in_cols, in_ld, C, 1, fp.pw, fp.ph));
-    } else {
-      DIP_CHECK(bf16 ? map_act5(&fp.tmA, in16, in_rows, in_cols, in_ld16, C, stride, bw, bh, false, true)
-                     : map_act5(&fp.tmA, in, in_rows, in_cols, in_ld, C, stride, bw, bh));
-    }
     if (do_fprop) {
-    fp.csize = fp.pair ? 1 : pick_csize(((out_w + bw - 1) / bw) * ((out_h + bh - 1) / bh), Np);
-    fp.tps = (fp.patch && fp.csize == 1) ? pick_tps() : 1;
-    fp.n_split = fp.pair ? 1 : fp.csize == 1 ? pick_nsplit(((out_w + bw - 1) / bw) * ((out_h + bh - 1) / bh), Np) : 1;
-    DIP_CHECK(map_w2(&fp.tmB, wp_f, k * k * Np, bf16 ? c_pad16 : c_pad, Np / fp.csize / fp.n_split, bf16));
+    DIP_CHECK(bf16 ? map_act5(&fp.tmA, in16, in_rows, in_cols, in_ld16, C, stride, bw, bh, true)
+                   : map_act5(&fp.tmA, in, in_rows, in_cols, in_ld, C, stride, bw, bh));
+    fp.n_split = pick_nsplit(((out_w + bw - 1) / bw) * ((out_h + bh - 1) / bh), Np);
+    DIP_CHECK(map_w2(&fp.tmB, wp_f, k * k * Np, bf16 ? c_pad16 : c_pad, Np / fp.n_split, bf16));
     DIP_CHECK(map_act3(&fp.tmD, out, out_h, out_w, N, N, bw, bh));
     fp.tiles_x = (out_w + bw - 1) / bw; fp.tiles_y = (out_h + bh - 1) / bh;
     fp.bw = bw; fp.bh = bh; fp.out_w = out_w; fp.out_h = out_h;
     fp.kh = fp.kw = k; fp.stride = stride; fp.offx = offx; fp.offy = offy;
     fp.bf16 = bf16 ? 1 : 0;
     fp.kblocks = bf16 ? c_pad16 / 64 : c_pad / 32;
-    fp.tail_mmas = bf16 ? ((C % 64 == 0) ? 4 : (C % 64 + 15) / 16) : ((C % 32 == 0) ? 4 : (C % 32 + 7) / 8);
     fp.n_mma = Np / fp.n_split; fp.n_chunks = (fp.n_mma + 31) / 32;
     fp.n_valid = N;
     fp.bias = nullptr; fp.stats = stats; fp.stats_ld = N;
@@ -325,9 +269,8 @@ struct ConvOp {
       const int gh = dg_out_h / 2, gw = dg_out_w / 2;
       pick_tile(gw, gh, &bw, &bh);
       dg = TcConvParams{};
-      DIP_CHECK(bf16 ? map_act5(&dg.tmA, dg_in16, dg_in_h, dg_in_w, N, N, 1, bw, bh, false, true)
+      DIP_CHECK(bf16 ? map_act5(&dg.tmA, dg_in16, dg_in_h, dg_in_w, N, N, 1, bw, bh, true)
                      : map_act5(&dg.tmA, dg_in, dg_in_h, dg_in_w, N, N, 1, bw, bh));
-      dg.csize = 1; dg.tps = 1;
       dg.n_split = pick_nsplit(4 * ((gw + bw - 1) / bw) * ((gh + bh - 1) / bh), crows);
       DIP_CHECK(map_w2(&dg.tmB, wp_d, k * k * crows, bf16 ? n_pad16 : n_pad, crows / dg.n_split, bf16));
       DIP_CHECK(map_act5(&dg.tmD, dg_out, dg_out_h, dg_out_w, dg_ld, C, 2, bw, bh));   // parity view of the padded gradient
@@ -344,35 +287,22 @@ struct ConvOp {
         }
       dg.bf16 = bf16 ? 1 : 0;
       dg.kblocks = bf16 ? n_pad16 / 64 : n_pad / 32;   // K = the N channels of dY
-      dg.tail_mmas = bf16 ? ((N % 64 == 0) ? 4 : (N % 64 + 15) / 16) : ((N % 32 == 0) ? 4 : (N % 32 + 7) / 8);
       dg.n_mma = crows / dg.n_split; dg.n_chunks = (dg.n_mma + 31) / 32;
       dg.bias = nullptr; dg.stats = nullptr; dg.stats_ld = 0;
       fit_stages(dg);
     } else if (has_dgrad) {
       pick_tile(dg_out_w, dg_out_h, &bw, &bh);
       dg = TcConvParams{};
-      if (k == 3 && patch_ok) {
-        bw = 8; bh = 16;
-        dg.patch = 1; dg.pw = bw + 2; dg.ph = bh + 2;
-        dg.pair = pick_pair((dg_out_w + bw - 1) / bw, (dg_out_h + bh - 1) / bh, crows);
-        if (dg.pair) dg.ph = 2 * bh + 2;
-        DIP_CHECK(bf16 ? map_act5(&dg.tmA, dg_in16, dg_in_h, dg_in_w, N, N, 1, dg.pw, dg.ph, false, true)
-                       : map_act5(&dg.tmA, dg_in, dg_in_h, dg_in_w, N, N, 1, dg.pw, dg.ph));
-      } else {
-        DIP_CHECK(bf16 ? map_act5(&dg.tmA, dg_in16, dg_in_h, dg_in_w, N, N, 1, bw, bh, false, true)
-                       : map_act5(&dg.tmA, dg_in, dg_in_h, dg_in_w, N, N, 1, bw, bh));
-      }
-      dg.csize = dg.pair ? 1 : pick_csize(((dg_out_w + bw - 1) / bw) * ((dg_out_h + bh - 1) / bh), crows);
-      dg.tps = (dg.patch && dg.csize == 1) ? pick_tps() : 1;
-      dg.n_split = dg.pair ? 1 : dg.csize == 1 ? pick_nsplit(((dg_out_w + bw - 1) / bw) * ((dg_out_h + bh - 1) / bh), crows) : 1;
-      DIP_CHECK(map_w2(&dg.tmB, wp_d, k * k * crows, bf16 ? n_pad16 : n_pad, crows / dg.csize / dg.n_split, bf16));
+      DIP_CHECK(bf16 ? map_act5(&dg.tmA, dg_in16, dg_in_h, dg_in_w, N, N, 1, bw, bh, true)
+                     : map_act5(&dg.tmA, dg_in, dg_in_h, dg_in_w, N, N, 1, bw, bh));
+      dg.n_split = pick_nsplit(((dg_out_w + bw - 1) / bw) * ((dg_out_h + bh - 1) / bh), crows);
+      DIP_CHECK(map_w2(&dg.tmB, wp_d, k * k * crows, bf16 ? n_pad16 : n_pad, crows / dg.n_split, bf16));
       DIP_CHECK(map_act3(&dg.tmD, dg_out, dg_out_h, dg_out_w, dg_ld, C, bw, bh));
       dg.tiles_x = (dg_out_w + bw - 1) / bw; dg.tiles_y = (dg_out_h + bh - 1) / bh;
       dg.bw = bw; dg.bh = bh; dg.out_w = dg_out_w; dg.out_h = dg_out_h;
       dg.kh = dg.kw = k; dg.stride = 1; dg.offx = dg.offy = dg_off;
       dg.bf16 = bf16 ? 1 : 0;
       dg.kblocks = bf16 ? n_pad16 / 64 : n_pad / 32;   // K = the N channels of dY
-      dg.tail_mmas = bf16 ? ((N % 64 == 0) ? 4 : (N % 64 + 15) / 16) : ((N % 32 == 0) ? 4 : (N % 32 + 7) / 8);
       dg.n_mma = crows / dg.n_split; dg.n_chunks = (dg.n_mma + 31) / 32;
       dg.bias = nullptr; dg.stats = nullptr; dg.stats_ld = 0;
       fit_stages(dg);
@@ -380,19 +310,17 @@ struct ConvOp {
     // ---- wgrad
     wg = TcWgradParams{};
     if (!do_wgrad) return 0;
-    wg.kp = wg_kp();
     wg.bf16 = bf16 ? 1 : 0;
-    wg.xshare = (stride == 1 && k == 3 && getenv("DIP_NO_XSHARE") == nullptr) ? 1 : 0;
     if (bf16) {
-      DIP_CHECK(map_act3(&wg.tmY, wg_dy16, wg_h, wg_w, N, N, wg.kp, 1, false, true));
-      DIP_CHECK(map_act5(&wg.tmX, in16, in_rows, in_cols, in_ld16, C, stride, wg.xshare ? wg.kp + k - 1 : wg.kp, 1, false, true));
+      DIP_CHECK(map_act3(&wg.tmY, wg_dy16, wg_h, wg_w, N, N, kWgradKp, 1, true));
+      DIP_CHECK(map_act5(&wg.tmX, in16, in_rows, in_cols, in_ld16, C, stride, kWgradKp, 1, true));
     } else {
-      DIP_CHECK(map_act3(&wg.tmY, wg_dy, wg_h, wg_w, N, N, wg.kp, 1, true));
-      DIP_CHECK(map_act5(&wg.tmX, in, in_rows, in_cols, in_ld, C, stride, wg.xshare ? wg.kp + k - 1 : wg.kp, 1, true));
+      DIP_CHECK(map_act3(&wg.tmY, wg_dy, wg_h, wg_w, N, N, kWgradKp, 1));
+      DIP_CHECK(map_act5(&wg.tmX, in, in_rows, in_cols, in_ld, C, stride, kWgradKp, 1));
     }
     wg.partial = partial;
     wg.kh = wg.kw = k; wg.stride = stride; wg.offx = offx; wg.offy = offy;
-    wg.px_blocks_x = (wg_w + wg.kp - 1) / wg.kp;
+    wg.px_blocks_x = (wg_w + kWgradKp - 1) / kWgradKp;
     wg.px_blocks = wg_h * wg.px_blocks_x;
     wg.c_chunks = bf16 ? c_pad16 / 64 : c_pad / 32;
     wg.n_cols = c_pad;
@@ -407,11 +335,6 @@ struct ConvOp {
     if (is_tc(prec)) {
       TcConvParams p = fp;
       p.bias = bias;
-      if (const char* e = getenv("DIP_DBG_SHIFT")) p.dbg_shift = atoi(e);
-      if (const char* e = getenv("DIP_DBG_BO")) p.dbg_bo = atoi(e);
-      if (const char* e = getenv("DIP_DBG_FLAGS")) p.dbg_flags = atoi(e);
-      if (const char* e = getenv("DIP_DBG_NMMA")) p.dbg_nmma = atoi(e);
-      if (const char* e = getenv("DIP_DBG_STAGES")) { const int st = atoi(e); if (st >= 1 && st < p.stages) p.stages = st; }
       TimeScope ts(timer, 0, alg_flops(), s);
       DIP_CUDA(tc_conv_launch(p, g_num_sms, s));
     } else {
@@ -446,19 +369,16 @@ struct ConvOp {
     if (dbg_skip) return 0;
     int ks;
     if (is_tc(prec)) {
-      // split-K CTAs add their tiles into one accumulator with vector reductions at the L2.  Plan-owned accumulator
-      // (wacc): zeroed by one memset per backward, unpacked to OIHW by one table kernel at the end of the backward pass.
-      // Single-op entry points: zero + launch + unpack here.
+      // every split-K work item writes its own partial slice.  Plan-owned partials (wacc) are summed and unpacked to
+      // OIHW by one table kernel at the end of the backward pass; single-op entry points reduce here.
       TcWgradParams p = wg;
-      p.atomic = 1;
       p.partial = wacc != nullptr ? wacc : partial;
-      if (wacc == nullptr) DIP_CUDA(cudaMemsetAsync(partial, 0, wacc_elems() * sizeof(float), s));
       {
         TimeScope ts(timer, 2, alg_flops(), s);
         DIP_CUDA(tc_wgrad_launch(p, s));
       }
       if (wacc != nullptr) return 0;
-      launch_wgrad_reduce(partial, 1, N, C, k, k, rot, c_pad, dw, s, Ctot, coff);
+      launch_wgrad_reduce(partial, p.ksplits, N, C, k, k, rot, c_pad, dw, s, Ctot, coff);
       DIP_CUDA(cudaGetLastError());
       return 0;
     } else {
@@ -518,10 +438,11 @@ __global__ void k_pack_table(const PackEntry* __restrict__ tab) {
     }
   }
 }
-// accumulators [tap][128][c_pad] of all tensor-core weight gradients -> OIHW gradients (one launch per backward pass)
+// partials [ks][tap][128][c_pad] of all tensor-core weight gradients -> OIHW gradients (one launch per backward pass);
+// the split-K slices are summed in index order, so the gradient is the same on every run
 struct UnpackEntry {
   const float* acc; float* dw;
-  int N, C, taps, rot, c_pad, Ctot, coff;
+  int N, C, taps, rot, c_pad, Ctot, coff, ks;
 };
 __global__ void k_wgrad_unpack_table(const UnpackEntry* __restrict__ tab) {
   pdl_enter();
@@ -529,7 +450,11 @@ __global__ void k_wgrad_unpack_table(const UnpackEntry* __restrict__ tab) {
   const int total = e.N * e.C * e.taps;   // dw elements this entry owns: (n, engine channel c, tap)
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     const int tap = i % e.taps, c = (i / e.taps) % e.C, n = i / (e.taps * e.C);
-    e.dw[((size_t)n * e.Ctot + (c + e.coff + e.rot) % e.Ctot) * e.taps + tap] = e.acc[((size_t)tap * 128 + n) * e.c_pad + c];
+    const size_t split = (size_t)e.taps * 128 * e.c_pad;
+    const float* src = e.acc + ((size_t)tap * 128 + n) * e.c_pad + c;
+    float v = 0.f;
+    for (int k = 0; k < e.ks; ++k) v += src[k * split];
+    e.dw[((size_t)n * e.Ctot + (c + e.coff + e.rot) % e.Ctot) * e.taps + tap] = v;
   }
 }
 struct CvtEntry {
@@ -1090,7 +1015,8 @@ static int upload_tables(dip_plan* P) {
     std::vector<UnpackEntry> up;
     for (ConvOp* op : P->convs) {
       if (!op->do_wgrad || op->wacc == nullptr) continue;
-      up.push_back(UnpackEntry{op->wacc, P->grads[op->p_w], op->N, op->C, op->k * op->k, op->rot, op->c_pad, op->Ctot, op->coff});
+      up.push_back(UnpackEntry{op->wacc, P->grads[op->p_w], op->N, op->C, op->k * op->k, op->rot, op->c_pad, op->Ctot, op->coff,
+                               op->wg.ksplits});
     }
     if ((int)up.size() != P->n_unpack) return fail("internal: unpack table size mismatch");
     DIP_CUDA(cudaMemcpy(P->d_unpack, up.data(), up.size() * sizeof(UnpackEntry), cudaMemcpyHostToDevice));
@@ -1177,10 +1103,9 @@ static const float* level_usrc(const dip_plan* P, int l) {
 
 // The persistent deep-level kernel (deep.cu) replaces the launches of levels >= deep_from (tensor-core precision, no
 // per-launch timers).  OPT-IN (DIP_DEEP=1): parity-green (tests/test_engine_gpu.py::test_deep_kernel_matches_launches) but
-// measured SLOWER than the launches it replaces on B200 -- forward 382 us vs 340 us, backward 745 us vs ~700 us of kernel time
-// (ncu), 314 vs 378 it/s end to end: the small kernels are bounded by their own prologue + a few memory round trips, not by
-// launch gaps, and one 256-thread CTA per SM (255 registers: the conv code lives in the same kernel) has an eighth of the
-// loads in flight that the stand-alone kernels have.  See DESIGN.md section 10.
+// not the default: the small kernels are bounded by their own prologue + a few memory round trips rather than by launch
+// gaps, and one 256-thread CTA per SM (the conv code lives in the same kernel) has far fewer loads in flight than the
+// stand-alone kernels.  Its speed on H100 has not been measured.
 static bool deep_on(const dip_plan* P) {
   const char* e = getenv("DIP_DEEP");   // read per call: the test switches it inside one process
   return e != nullptr && e[0] == '1' && P->desc.precision == DIP_PRECISION_TF32 && !P->timer.on && P->n_deep_fwd > 0 &&
@@ -1334,7 +1259,8 @@ static GradSrc src_upadj(const float* d, int ld, int bilinear) { GradSrc s{}; s.
 // stream has the higher priority, so that the wgrad overlaps the HBM-bound kernels that follow the dgrad instead of
 // delaying it.  (DIP_WGRAD_FIRST=1: the old order, for A/B runs.)
 static int defer_level() {
-  // measured (profiles/r01_matrix_wgrad_schedule.txt): 347.5 it/s without deferral, 352.3 with the level-0/1 wgrads deferred
+  // weight gradients of the levels above this index are deferred until the backward pass reaches it, so that they run
+  // beside the deeper levels' launches
   static const int lv = getenv("DIP_DEFER_WGRAD") ? atoi(getenv("DIP_DEFER_WGRAD")) : 2;   // 0: no deferral
   return lv;
 }
@@ -1524,10 +1450,7 @@ static DeepOp deep_wgrad(dip_plan* P, const ConvOp& op, int sync = 1) {
   DeepOp o;
   o.type = DO_WGRAD; o.sync = sync;
   o.u.wg = op.wg;
-  o.u.wg.atomic = 1;
   o.u.wg.partial = op.wacc;
-  const int cap = P->deep_grid / op.k;   // kh * ksplits CTAs must fit the deep grid
-  if (o.u.wg.ksplits > cap) o.u.wg.ksplits = cap;
   while (tc_wgrad_smem_bytes(o.u.wg) > deep_dyn_smem() && o.u.wg.stages > 1) o.u.wg.stages--;
   return o;
 }
@@ -1625,7 +1548,6 @@ static int plan_backward(dip_plan* P, const float* dout, cudaStream_t s) {
   int nl = 0;
   P->deferred.clear();
   DIP_CUDA(cudaMemsetAsync(P->acc_bwd, 0, P->acc_bwd_n * sizeof(double), s));
-  if (P->n_unpack > 0) DIP_CUDA(cudaMemsetAsync(P->wacc_base, 0, P->wacc_bytes, s));
   P->side_on = getenv("DIP_NO_SIDE") == nullptr;
   Level& v0 = P->lv[0];
   // RGB head backward (sigmoid', dgrad 3->128, wgrad, bias grad) is fused into the BN backward of the last stage
@@ -1644,7 +1566,7 @@ static int plan_backward(dip_plan* P, const float* dout, cudaStream_t s) {
   if (P->n_unpack > 0) {
     HBM_T(&P->timer, H_WGRAD_REDUCE, 1, 2.0 * (double)P->wacc_bytes, s,
           launch_k(k_wgrad_unpack_table, dim3(64, P->n_unpack), dim3(256), 0, s, 1, P->d_unpack));
-    nl += 2;   // + the accumulator memset
+    nl += 1;
   }
   DIP_CUDA(cudaGetLastError());
   P->launches_bwd = nl;

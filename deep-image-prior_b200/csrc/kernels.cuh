@@ -1,4 +1,4 @@
-// Launch wrappers of the HBM-bound kernels of the dip-b200 engine (kernels_mem.cu, conv_simt.cu).
+// Launch wrappers of the HBM-bound kernels of the dip engine (kernels_mem.cu, conv_simt.cu).
 // All activations are fp32 NHWC; "ld" is the channel stride of a buffer in floats.  Precision mode bf16 adds bf16 twins (Twin) of
 // the tensors the tensor-core kernels read; everything these kernels compute with stays fp32.
 #pragma once
@@ -9,6 +9,7 @@
 namespace dip {
 
 static constexpr float kBnEps = 1e-5f;
+static constexpr long long kNumSms = 132;      // H100 SXM: grid caps of the grid-stride kernels (a few blocks per SM)
 static constexpr float kLreluSlope = 0.2f;
 // fp64 accumulators are spread one per 128-byte line (stride in doubles): hundreds of blocks add to them at the end of
 // every reduction kernel: neighbouring channels must not share an L2 atomic unit, and each accumulator is split into
@@ -36,7 +37,7 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 __device__ __forceinline__ void pdl_enter() { pdl_trigger(); pdl_wait(); }
 #endif
 inline bool pdl_enabled() {
-  static const bool on = getenv("DIP_PDL") != nullptr;  // measured: no gain inside the CUDA graph (296 vs 299 it/s) -> opt-in
+  static const bool on = getenv("DIP_PDL") != nullptr;  // opt-in: the step is replayed as a CUDA graph anyway
   return on;
 }
 // kernel<<<grid, block, smem, s>>>(args...) with the programmatic-serialization attribute (and an optional cluster)

@@ -141,7 +141,7 @@ static VecGeom vec_geom(int C, long long nitems) {
   if (g.PPB < 1) g.PPB = 1;
   g.threads = g.VL * g.PPB;
   long long nb = (nitems + g.PPB - 1) / g.PPB;
-  const long long cap = g.VL >= 8 ? 148LL * 8 : 148LL * 2;
+  const long long cap = g.VL >= 8 ? kNumSms * 8 : kNumSms * 2;
   g.blocks = static_cast<int>(nb < cap ? nb : cap);
   if (g.blocks < 1) g.blocks = 1;
   return g;
@@ -151,9 +151,7 @@ static VecGeom vec_geom(int C, long long nitems) {
 // Threads are laid out tid = slot * VL + v.  For VL in {1,2,4,8,16} the lanes that share v are first folded with
 // warp shuffles (blockDim is then a multiple of 32).  wid[k] = valid channels of dst[k].
 // The accumulators live one per 128-byte line (kAccS): hundreds of blocks add to the same 2*C addresses at the end of a
-// single-wave kernel, and neighbouring channels sharing an L2 atomic unit cost ~0.3 ms per iteration.  (Per-block
-// partials + last-block sum, cluster/DSMEM pre-reduction and replicated accumulators were all measured slower:
-// profiles/r01_experiments.md.)
+// single-wave kernel, and neighbouring channels sharing an L2 atomic unit serialise their atomics.
 template <int K>
 __device__ __forceinline__ void block_reduce_atomic(float4 (&acc)[K], int VL, int PPB, double* const* dst, const int* wid) {
   extern __shared__ float4 red_smem[];
@@ -215,7 +213,7 @@ static void fit_grid(VecGeom& g, Kern kernel, size_t smem) {
   } else {
     per_sm = it->second;
   }
-  const int cap = 148 * per_sm;
+  const int cap = kNumSms * per_sm;
   if (g.blocks > cap) g.blocks = cap;
 }
 
@@ -271,7 +269,7 @@ __global__ void __launch_bounds__(256) k_cast_bf16(const float* __restrict__ x, 
 void launch_cast_bf16(const float* x, int ld, int c, long long npix, Twin t, cudaStream_t s) {
   const long long n4 = npix * (c / 4);
   long long blocks = (n4 + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > kNumSms * 8) blocks = kNumSms * 8;
   if (blocks < 1) blocks = 1;
   launch_k(k_cast_bf16, dim3((unsigned)blocks), dim3(256), 0, s, 1, x, ld, c / 4, n4, t);
 }
@@ -389,7 +387,7 @@ __global__ void __launch_bounds__(256) k_bn_act_head(const float* __restrict__ r
 void launch_bn_act_head(const float* raw, BnRef bn, int H, int W, HeadRef head, cudaStream_t s) {
   const int npix = H * W;
   int blocks = (npix + 7) / 8;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > kNumSms * 8) blocks = kNumSms * 8;
   launch_k(k_bn_act_head, dim3(blocks), dim3(256), 0, s, 1, raw, bn, npix, head);
 }
 
@@ -706,7 +704,7 @@ __global__ void k_head_dlogit(const float* __restrict__ dout, const float* __res
 }
 void launch_head_dlogit(const float* dout, const float* outv, int K, int npix, float* dl4, cudaStream_t s, int sigmoid) {
   int blocks = (npix + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > kNumSms * 8) blocks = kNumSms * 8;
   launch_k(k_head_dlogit, dim3(blocks), dim3(256), 0, s, 1, dout, outv, K, npix, dl4, sigmoid);
 }
 
@@ -948,8 +946,7 @@ __device__ __forceinline__ void d_cat_bwd_reduce(const float* __restrict__ pcat,
   const CatBwdCoef cf = cat_bwd_coef(bn_cat, v);
   const int Wp = W + 2;
   float4 acc[2] = {f4zero(), f4zero()};
-  // (the row-segment loop of the BN backward kernels was measured SLOWER here: 53.6 -> 65.9 us at 512x512 -- with 33 lanes
-  // per pixel a unit is only 14 pixels and these two kernels already run at 5.2 - 6.1 TB/s)
+  // (no row-segment loop as in the BN backward kernels: with 33 lanes per pixel a unit would be only 14 pixels)
   item_loop<DIP_U_CATBWD>(slot < PPB ? blockIdx.x * PPB + slot : H * W, gridDim.x * PPB, H * W,
                [&](int p) {
                  RedItem it;
@@ -1229,7 +1226,7 @@ void launch_skinny_fwd(const float* x, int ldx, int x_rs, const float* w, const 
                        int W, float* y, int mode, double* stats, cudaStream_t s, int cw) {
   const int PPB = C >= 32 ? 64 : 256 / (C / 4);   // pixels per block and trip (wide path: 64 whatever the depth)
   long long nb = (static_cast<long long>(H) * W + PPB - 1) / PPB;
-  if (nb > 148 * 8) nb = 148 * 8;
+  if (nb > kNumSms * 8) nb = kNumSms * 8;
   launch_red(k_skinny_fwd, static_cast<int>(nb), 256, 2 * 256 * sizeof(float4) + 2 * 4 * sizeof(double), s, x, ldx, x_rs, w, b, C, N, H, W,
                   y, mode, stats, cw > 0 ? cw : C);
 }
@@ -1318,14 +1315,19 @@ __global__ void k_mse(const float* __restrict__ out, const float* __restrict__ t
   if (threadIdx.x < 32) {
     float t = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
     for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-    if (threadIdx.x == 0) atomicAdd(loss + (it_dev != nullptr ? *it_dev : 0), static_cast<double>(t) * static_cast<double>(inv_n));
+    // each block's term rounded to a multiple of 2^-48: every partial sum below 32 is then exact in fp64, so the loss does
+    // not depend on the order of the atomics; the rounding is <= 2^-49 per block, far below the fp32 error of `t` itself
+    if (threadIdx.x == 0) {
+      const double v = static_cast<double>(t) * static_cast<double>(inv_n);
+      atomicAdd(loss + (it_dev != nullptr ? *it_dev : 0), ldexp(rint(ldexp(v, 48)), -48));
+    }
   }
 }
 void launch_mse(const float* out, const float* target, const float* mask, int C, int HW, double* loss, float* dout,
                 const int* it_dev, cudaStream_t s) {
   const long long n = static_cast<long long>(C) * HW;
   int blocks = static_cast<int>((n + 255) / 256);
-  if (blocks > 148 * 4) blocks = 148 * 4;
+  if (blocks > kNumSms * 4) blocks = kNumSms * 4;
   launch_k(k_mse, dim3(blocks), dim3(256), 0, s, 1, out, target, mask, C, HW, loss, dout, it_dev);
 }
 
@@ -1372,7 +1374,7 @@ void launch_noise(const float* z0, float* z, float sigma, uint64_t seed, uint64_
                   cudaStream_t s) {
   const size_t n4 = n / 4;
   int blocks = static_cast<int>((n4 + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > kNumSms * 16) blocks = kNumSms * 16;
   launch_k(k_noise, dim3(blocks), dim3(256), 0, s, 1, z0, z, sigma, seed, offset, it_dev, n4);
 }
 // Fused runner input: z = z0 + sigma * N(0,1) written straight into the reflection-padded NHWC level-0 buffer (k_noise +

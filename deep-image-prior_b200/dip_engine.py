@@ -1,7 +1,7 @@
 """ctypes binding of libdip.so (C ABI declared in include/dip.h).
 
 This is the only place where Python touches the native engine.  PyTorch is used for device memory, streams and
-autograd plumbing; every FLOP of the hot path runs in the hand-written sm_100a kernels of libdip.so.
+autograd plumbing; every FLOP of the hot path runs in the hand-written sm_90a kernels of libdip.so.
 The library is mandatory: there is no CPU or eager-PyTorch fallback for the accelerated path.
 """
 import ctypes
@@ -52,7 +52,7 @@ ABI_SYMBOLS = [
 
 
 def build(verbose=False):
-    """Compile libdip.so in-tree with nvcc for sm_100a (no GPU needed)."""
+    """Compile libdip.so in-tree with nvcc for sm_90a (no GPU needed)."""
     out = subprocess.run([os.path.join(_HERE, "build.sh")], capture_output=True, text=True)
     if verbose or out.returncode != 0:
         print(out.stdout)
@@ -153,7 +153,7 @@ class Plan:
             assert all(len(x) == num_scales for x in per_scale) and num_scales <= 8
             channels, skip_channels = 0, 0
         if not torch.cuda.is_available():
-            raise RuntimeError("dip-b200 needs a CUDA device (sm_100a); none is visible")
+            raise RuntimeError("dip-b200 needs a CUDA device (sm_90a); none is visible")
         self.device = torch.device(device if device is not None else "cuda:%d" % torch.cuda.current_device())
         # bilinear: one flag for every scale, or a per-scale sequence (flash-no-flash.ipynb c8)
         if isinstance(bilinear, (list, tuple)):

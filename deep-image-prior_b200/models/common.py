@@ -2,7 +2,7 @@
 
 The blocks are ordinary torch modules because they double as the parameter holders / state_dict layout of the
 network; on the accelerated path their forward() is never called -- SkipNet (models/skip.py) hands the whole graph to
-the sm_100a engine instead.
+the sm_90a engine instead.
 """
 import numpy as np
 import torch

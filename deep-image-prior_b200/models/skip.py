@@ -3,7 +3,7 @@
 The returned object is an nn.Sequential whose children, parameter names, parameter order and initialisation RNG order
 are those of the reference (so state_dict()s are interchangeable and torch.manual_seed(s) gives identical weights), but
 calling it does NOT interpret the module tree: for the configurations of BASELINE.json the whole forward + backward runs
-in the hand-written sm_100a engine (libdip.so) through one autograd node.  There is no silent fallback: unsupported
+in the hand-written sm_90a engine (libdip.so) through one autograd node.  There is no silent fallback: unsupported
 configurations or CPU tensors raise unless the caller opts in to stock-torch execution with
 `models.allow_torch_execution(True)` (used by the CPU tests that compare the tree with the reference's).
 """
@@ -72,7 +72,7 @@ class SkipNet(nn.Sequential):
         self._dip_anchor = None
         self._dip_generation = 0     # bumped by every engine forward (guards backward against stale activations)
         self._dip_active_plan = None
-        # 'tf32' (tcgen05 kind::tf32, default) | 'fp32' (exact CUDA-core parity mode) | 'bf16' (tcgen05 kind::f16 on bf16
+        # 'tf32' (wgmma tf32, default) | 'fp32' (exact CUDA-core parity mode) | 'bf16' (wgmma on bf16
         # operands, fp32 accumulate / master weights / BatchNorm / Adam: BASELINE.json configs[2])
         self.precision = 'tf32'
 

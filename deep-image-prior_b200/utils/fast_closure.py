@@ -3,7 +3,7 @@
 The denoising notebook's closure (denoising.ipynb c10:8-56) does, every iteration, three device->host copies of the
 3 x H x W output for skimage's compare_psnr, and `last_net = [x.detach().cpu() for x in net.parameters()]` -- 112 more
 copies with a sync each.  None of that can be made cheap from below while the cell text stays as it is (the cost is in
-`.cpu()` itself), so the unmodified notebook runs at ~90 it/s on a B200 however fast the network is.  This module
+`.cpu()` itself), so the unmodified notebook is bounded by those host round trips however fast the network is.  This module
 keeps the SAME logic -- perturbed input, EMA `out_avg`, PSNR_noisy / PSNR_gt / PSNR_gt_sm, back-tracking to the last
 good parameters when PSNR_noisy drops by more than 5 dB -- but keeps the quantities on the device:
 

@@ -1,4 +1,4 @@
-/* dip.h -- C ABI of libdip.so, the B200-native deep-image-prior hot-path engine.
+/* dip.h -- C ABI of libdip.so, the H100-native deep-image-prior hot-path engine.
  *
  * The reference (DmitryUlyanov/deep-image-prior) has no FFI: its hot path sits behind plain Python call sites.
  * Every entry point below names the reference call site it replaces (file:line into the reference repo).
@@ -23,9 +23,9 @@ typedef struct dip_plan dip_plan;
 typedef struct dip_adam dip_adam;
 typedef void* dip_stream_t; /* cudaStream_t */
 
-enum { DIP_PRECISION_TF32 = 0, /* tcgen05 kind::tf32 convolutions, fp32 accumulate (cuDNN's default fp32 mode) */
+enum { DIP_PRECISION_TF32 = 0, /* wgmma tf32 convolutions, fp32 accumulate (cuDNN's default fp32 mode) */
        DIP_PRECISION_FP32 = 1, /* exact-fp32 CUDA-core convolutions (parity mode) */
-       DIP_PRECISION_BF16 = 2  /* tcgen05 kind::f16 convolutions on bf16 operands (activations, gradients and weights rounded
+       DIP_PRECISION_BF16 = 2  /* wgmma bf16 convolutions on bf16 operands (activations, gradients and weights rounded
                                   to bf16 where a convolution reads them), fp32 accumulate; fp32 master weights, BatchNorm,
                                   loss and Adam (BASELINE.json configs[2]: "super-resolution ... bf16") */ };
 

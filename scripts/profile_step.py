@@ -1,4 +1,4 @@
-"""Runs N iterations of the device runner (for ncu launch lists / captures). usage: profile_step.py [iters] [H] [W]
+"""Runs N iterations of the device runner (a workload to profile, e.g. with torch.profiler). usage: profile_step.py [iters] [H] [W]
 env: DIP_PROF_CS=4|128 (skip channels), DIP_PROF_MODE=bilinear|nearest, DIP_PROF_SR=1 (x4 Lanczos-2 downsampler in the loss),
 DIP_PROF_MASK=1 (masked MSE), DIP_PROF_PREC=tf32|fp32|bf16"""
 import os, sys, torch

@@ -17,7 +17,7 @@ def pytest_configure(config):
         torch.set_num_threads(min(8, os.cpu_count() or 1))
     except Exception:
         pass
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200, sm_100a)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100, sm_90a)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -1,6 +1,6 @@
 """Precision mode 'bf16' (BASELINE.json configs[2]: "super-resolution x4 ... bf16") on the GPU.
 
-What bf16 means here (DESIGN.md section 3, include/dip.h DIP_PRECISION_BF16): the wide convolutions run as tcgen05 kind::f16
+What bf16 means here (DESIGN.md section 3, include/dip.h DIP_PRECISION_BF16): the wide convolutions run as wgmma
 MMAs on bf16 operands -- their input, their weight and the incoming gradient are rounded to bf16 where the tensor-core
 kernels read them -- with fp32 accumulation; master weights, biases, BatchNorm, activations, up-sampling, the skinny skip
 convs, the head, the loss and Adam stay fp32.  The reference has no bf16 path; the checker is
@@ -140,7 +140,7 @@ def check_layers(tag, cfg, plan, params, dgrads):
 
 @pytest.mark.parametrize("kind", ["snail", "restoration_kate"])
 def test_bf16_layers_per_scale_widths(kind):
-    """The bf16 kernels on per-scale widths (K blocks with 8 / 16 / 32 valid channels of 64, UMMA N = 16 .. 128) and, for
+    """The bf16 kernels on per-scale widths (K blocks with 8 / 16 / 32 valid channels of 64, wgmma N = 32 .. 128) and, for
     restoration.ipynb's kate network, the stride-1 first down conv behind downsample_mode='avg': layer-local, exact-level."""
     if kind == "snail":      # denoising.ipynb c8:13-23
         cfg = O.SkipConfig(in_channels=3, channels=[8, 16, 32, 64, 128], skip_channels=[0, 0, 0, 4, 4])

@@ -1,7 +1,7 @@
-"""P1 (kernel tier): the tcgen05 / SIMT convolution kernels behind the C ABI vs torch-CPU fp64 (SURVEY.md 7.4).
+"""P1 (kernel tier): the wgmma / SIMT convolution kernels behind the C ABI vs torch-CPU fp64 (SURVEY.md 7.4).
 
 Tolerances: fp32 mode <= 2e-6 relative Frobenius error; tf32 mode <= 2e-3 (10-bit mantissa operands, fp32 accumulate);
-bf16 mode (precision 2, tcgen05 kind::f16): the reference is evaluated on the operands ROUNDED TO BF16 (what the kernel
+bf16 mode (precision 2, wgmma bf16): the reference is evaluated on the operands ROUNDED TO BF16 (what the kernel
 reads), products and sums in fp64 -> only the fp32 accumulation differs: <= 2e-5.
 """
 import pytest
@@ -38,10 +38,10 @@ CASES = [
     (128, 3, 1, 24, 36, 0),
     (132, 3, 1, 2, 2, 4),
     (128, 3, 1, 64, 128, 0),
-    (128, 3, 1, 256, 256, 0),     # >= 2 waves of tiles: cluster multicast of the weight tile
+    (128, 3, 1, 256, 256, 0),     # >= 2 waves of tiles: persistent CTAs walk several tiles each
     (132, 3, 1, 200, 312, 4),
     (128, 1, 1, 256, 512, 0),
-    (128, 3, 1, 270, 150, 0),     # tile-pair mode (>= 2 x 148 tiles of 8 x 16) with ragged right / bottom tiles and an odd tile-row count
+    (128, 3, 1, 270, 150, 0),     # several waves of tiles with ragged right / bottom tiles
 ]
 
 

@@ -337,7 +337,7 @@ def test_inpainting_closure_through_modules_vs_golden(prec):
 def test_deep_kernel_matches_launches():
     """DIP_DEEP=1: levels >= 2 run as ONE persistent kernel per pass (deep.cu: op list + grid-wide barriers, the same device
     code as the stand-alone kernels).  It must reproduce the launch-by-launch path: outputs, every gradient, and a few runner
-    iterations.  (Opt-in: measured slower than the launches it replaces, see DESIGN.md section 10.)"""
+    iterations.  (Opt-in, not the default: see DESIGN.md section 9.)"""
     import dip_engine as de
     H, W = 64, 96
     cfg, params, z0, target, _ = make_problem(H, W, "bilinear")

@@ -205,7 +205,7 @@ def run_sr_full_budget(prec):
 def test_sr_zebra_2000_iterations_vs_reference_runs(prec):
     """BASELINE config 3 at its full budget (the real zebra pair): end-of-run PSNR_HR / PSNR_LR (means over the last 50
     iterations) of the engine vs two runs of the unmodified reference; same acceptance band as the denoising test.
-    prec = 'bf16' is BASELINE's wording for this configuration (tcgen05 kind::f16 convolutions on bf16 operands)."""
+    prec = 'bf16' is BASELINE's wording for this configuration (wgmma convolutions on bf16 operands)."""
     rows, rec, refs = run_sr_full_budget(prec)
     assert abs(rec["loss"][0] - float(refs[0]["loss"][0])) < (1e-3 if prec == "tf32" else 5e-3)
     for key in ("psnr_LR", "psnr_HR"):
