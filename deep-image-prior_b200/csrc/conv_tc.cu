@@ -8,9 +8,10 @@
 //                       warp 3     loads the bias
 //                       warps 4-7  one warpgroup: wgmma on the 128-pixel tile (two m64 halves, fp32 accumulators in
 //                                  registers), then the epilogue: +bias -> swizzled smem -> per-channel BN statistics -> TMA store
-//   tc_wgrad_kernel : weight gradient, split-K over work items (tap, pixel range), one partial slice per item.  dY and X arrive pixel-major from NHWC
-//                     activations; wgmma reads tf32 operands K-major only, so the warpgroup transposes each stage into
-//                     K-major 128-byte-swizzled tiles (double-buffered) before it multiplies.
+//   tc_wgrad_kernel : weight gradient, split-K over work items (tap, pixel range), one partial slice per item.  dY and X arrive
+//                     pixel-major from NHWC activations.  tf32: warps 4-7 read dY straight into wgmma A registers; wgmma reads
+//                     a shared-memory tf32 B K-major only, so warps 1-3 transpose X into a double-buffered K-major tile while
+//                     the previous block multiplies.  bf16: the warpgroup transposes both operands, then multiplies.
 //   Both are templated on the operand type: tf32 on fp32 tensors (tc_conv_kernel / tc_wgrad_kernel) and bf16 on bf16 twins
 //   (tc_conv_kernel_bf16 / tc_wgrad_kernel_bf16, precision mode bf16); accumulators and outputs are fp32 in both.
 #include "conv_tc.cuh"
@@ -283,25 +284,207 @@ __global__ void __launch_bounds__(kNumThreads, 1) tc_conv_kernel_bf16(const __gr
 struct SmemCtlW {
   uint64_t full[8];
   uint64_t empty[8];
+  uint64_t bt_full[2];    // tf32: the transposer warps have written Bt buffer i
+  uint64_t bt_empty[2];   // tf32: the wgmmas that read Bt buffer i have completed
 };
 
-// Consumer warpgroup of the wgrad kernel, NT = accumulator columns per tap (p.n_cols).  Per pixel block: transpose the
-// pixel-major stage (dY: 128 channels, X: NT channels, kWgradKp pixels each, 128-byte swizzled rows of 32 fp32 / 64 bf16 channels)
-// into K-major swizzled tiles At [128 rows][kWgradKp pixels] and Bt [NT rows][kWgradKp pixels], then D[n][c] += At * Bt^T.
-template <bool BF16, int NT>
-__device__ __forceinline__ void tc_wgrad_consumer(const TcWgradParams& p, SmemCtlW* ctl, uint8_t* smem, int stage_bytes,
-                                                  uint8_t* tbase, int items) {
-  constexpr int KE = BF16 ? 64 : 32;                 // channels per 128-byte source row
-  constexpr int E = BF16 ? 2 : 4;                    // bytes per element
+// Shared-memory bytes of one transposed operand buffer: [At, bf16 only: 128 rows][Bt: n_cols rows], 128 bytes a row.
+__host__ __device__ constexpr int wgrad_tbuf_bytes(bool bf16, int n_cols) {
+  return (bf16 ? kTileM * 128 : 0) + round1024(n_cols * 128);
+}
+
+// The tf32 weight gradient, per 32-pixel block of a work item: D[n][c] += dY[px][n]^T * X[px][c] over the block's pixels.
+// A = dY^T (M = the 128 output channels) is read straight from the pixel-major TMA stage into registers (register-A wgmma);
+// B = X^T must be K-major in shared memory, so warps 1-3 transpose the X stage into a double-buffered Bt tile while warps
+// 4-7 run the wgmmas of the previous block.
+//
+// K order: inside every k8 step (pixels 8kk .. 8kk+7) K position j holds pixel 8kk + 2j for j < 4 and 8kk + 2(j-4) + 1 for
+// j >= 4 -- even pixels first.  A and B use the same order, so the product is unchanged (the accumulation order inside one
+// wgmma is the hardware's); it is the order that makes both the A-fragment loads and the transpose conflict-free (below).
+//
+// Stage layout (both operands): 128-byte rows of 32 fp32 channels, one row per pixel, chunks of 32 rows (4096 B) per 32
+// channels, 16-byte group q of row px stored at slot q ^ (px & 7) (the TMA 128-byte swizzle).
+
+// Warps 1-3 (96 threads): X stage -> Bt[NT rows = channels][32 pixels in the K order above], K-major SW128.
+// A unit is 4 channels (group c4) x 4 pixels (8kk + e + 2i, i = 0..3): four LDS.128 (one per pixel, 4 channels each), a 4x4
+// register transpose, four STS.128 (one per channel, 4 pixels each) into 16-byte group 2kk + e of the channel's Bt row.
+// Bank argument: the 8 lanes that share a 128-bit shared-memory wavefront are b = lane & 7, with e = b0, c4 bits 1,2 = b1,b2,
+// and kk = (b1 ^ o0) | (b2 ^ o1) << 1, c4 bit 0 = o2 for the lane-independent unit index o.  An LDS.128 of pixel 8kk + e + 2i
+// hits slot (c4 & 7) ^ (e + 2i), whose bits are (o2 ^ b0, b1 ^ i0, b2 ^ i1): 8 distinct slots over b.  An STS.128 of channel
+// 4 c4 + r hits slot (2kk + e) ^ (4 (c4 & 1) + r), bits (b0 ^ r0, b1 ^ o0 ^ r1, b2 ^ o1 ^ o2): 8 distinct slots over b.
+// Both are conflict-free.  Units cover (c4 < NT / 4) x (kk < 4) x (e < 2) exactly once.
+template <int NT>
+__device__ __forceinline__ void tc_wgrad_transposer(const TcWgradParams& p, SmemCtlW* ctl, uint32_t stage_base, int stage_bytes,
+                                                    uint32_t bt_base, int items) {
+  constexpr int kBt = wgrad_tbuf_bytes(false, NT);
+  constexpr int kUnitsO = ((NT + 31) / 32) * 8;        // values of o (8 lanes each) covering round32(NT) channels
+  constexpr int kIters = (kUnitsO + 11) / 12;          // 12 groups of 8 lanes in warps 1-3
+  constexpr int y_bytes = 4 * kWgradKp * 128;          // dY: 128 channels = 4 chunks
+  const int tt = threadIdx.x - 32;
+  const int lane = threadIdx.x & 31;
+  const int b = tt & 7, b0 = b & 1, b1 = (b >> 1) & 1, b2 = b >> 2;
+  // per unit: source offset of pixel 8kk + e (+ 2i: 256 i bytes, slot ^ 2i), Bt offset of channel 4 c4 (+ r: 128 r bytes, slot ^ r)
+  uint32_t src[kIters], dst[kIters], sq[kIters], dq[kIters];
+  bool ok[kIters];
+#pragma unroll
+  for (int it = 0; it < kIters; ++it) {
+    const int o = (tt >> 3) + 12 * it;
+    const int kk = (b1 ^ (o & 1)) | ((b2 ^ ((o >> 1) & 1)) << 1);
+    const int c4 = (o >> 3) * 8 + b2 * 4 + b1 * 2 + ((o >> 2) & 1);
+    ok[it] = o < kUnitsO && c4 < NT / 4;
+    src[it] = y_bytes + (c4 >> 3) * (kWgradKp * 128) + (8 * kk + b0) * 128;
+    sq[it] = (c4 & 7) ^ b0;                          // slot of pixel 8kk + e before the ^ 2i
+    dst[it] = c4 * 4 * 128;
+    dq[it] = (2 * kk + b0) ^ ((c4 & 1) << 2);        // slot of channel 4 c4 before the ^ r
+  }
+  int stage = 0, tb = 0;
+  uint32_t phase = 0, tphase = 0;
+  for (int item = blockIdx.x; item < items; item += gridDim.x) {
+    const int ks = item % p.ksplits;
+    const int blk0 = static_cast<int>((static_cast<long long>(p.px_blocks) * ks) / p.ksplits);
+    const int blk1 = static_cast<int>((static_cast<long long>(p.px_blocks) * (ks + 1)) / p.ksplits);
+    for (int blk = blk0; blk < blk1; ++blk) {
+      mbar_wait(&ctl->full[stage], phase);
+      mbar_wait(&ctl->bt_empty[tb], tphase ^ 1);
+      const uint32_t sx = stage_base + stage * stage_bytes;
+      const uint32_t bt = bt_base + tb * kBt;
+#pragma unroll
+      for (int it = 0; it < kIters; ++it) {
+        if (ok[it]) {
+          uint4 v[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) v[i] = lds128(sx + src[it] + 256 * i + ((sq[it] ^ (2 * i)) << 4));
+          sts128(bt + dst[it] + ((dq[it] ^ 0) << 4), v[0].x, v[1].x, v[2].x, v[3].x);
+          sts128(bt + dst[it] + 128 + ((dq[it] ^ 1) << 4), v[0].y, v[1].y, v[2].y, v[3].y);
+          sts128(bt + dst[it] + 256 + ((dq[it] ^ 2) << 4), v[0].z, v[1].z, v[2].z, v[3].z);
+          sts128(bt + dst[it] + 384 + ((dq[it] ^ 3) << 4), v[0].w, v[1].w, v[2].w, v[3].w);
+        }
+      }
+      fence_proxy_async_smem();                  // the Bt writes are read by wgmma (async proxy)
+      mbar_arrive(&ctl->bt_full[tb]);            // one arrival per transposer thread
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&ctl->empty[stage]);
+      if (++stage == p.stages) { stage = 0; phase ^= 1; }
+      tb ^= 1;
+      if (tb == 0) tphase ^= 1;
+    }
+  }
+}
+
+// Warps 4-7 (one warpgroup): register-A wgmmas on the dY stage and the Bt tile, fp32 accumulators [2 m64 halves][NT / 2].
+// The A fragments of block n+1 are loaded while the wgmmas of block n run (two register sets, fa / fb), except at NT = 160,
+// where NT accumulators + 64 fragment registers do not fit in 255 registers, and inside the persistent deep-level kernel
+// (deep.cu), whose other ops already hold registers: there the loads wait for the wgmmas.
+template <int NT, bool DOUBLE>
+__device__ __forceinline__ void tc_wgrad_mma(const TcWgradParams& p, SmemCtlW* ctl, uint32_t stage_base, int stage_bytes,
+                                             uint32_t bt_base, int items) {
+  constexpr int kBt = wgrad_tbuf_bytes(false, NT);
+  constexpr bool kDouble = DOUBLE && NT <= 136;
+  const int et = threadIdx.x - 128;
+  const int w = et >> 5, lane = et & 31, g = lane >> 2, t = lane & 3;
+  const int taps = p.kh * p.kw;
+  // A fragment of k8 step kk, m64 half h: a[0] = (channel n, pixel 8kk + 2t), a[1] = (n + 8, same), a[2] / a[3] = pixel + 1,
+  // n = 64h + 16w + g.  Channel n sits in chunk n / 32 = 2h + w / 2, 16-byte group q = 4 (w & 1) + g / 4 (+ 2 for n + 8),
+  // word g & 3; pixel 8kk + 2t + e in row 8kk + 2t + e, slot q ^ (2t + e).  Bank argument: over a warp (g, t) the slot takes
+  // 8 distinct values (bit 0 = g / 4 ^ e, bits 1-2 = t ^ (2 (w & 1) + hi), hi = 1 for n + 8) and the word g & 3 four more:
+  // 32 distinct banks.
+  uint32_t aoff[4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    const int hi = r & 1, e = r >> 1;
+    const int q = 4 * (w & 1) + (g >> 2) + 2 * hi, px = 2 * t + e;
+    aoff[r] = (w >> 1) * (kWgradKp * 128) + px * 128 + ((q ^ px) << 4) + (g & 3) * 4;
+  }
+  auto load_a = [&](uint32_t (&f)[8][4], uint32_t sy) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+        for (int r = 0; r < 4; ++r) f[4 * h + kk][r] = lds32(sy + aoff[r] + h * 2 * (kWgradKp * 128) + kk * 1024);
+  };
+  int stage = 0, tb = 0;
+  uint32_t phase = 0, tphase = 0;
+  bool pending = false;   // the previous block's Bt buffer is still to be handed back
+  float acc[2][NT / 2];
+  uint32_t fa[8][4], fb[8][4];
+  // one pixel block: the wgmmas on `cur`, then (while they run) the A fragments of the next block into `nxt`
+  auto step = [&](uint32_t (&cur)[8][4], uint32_t (&nxt)[8][4], bool more) {
+    mbar_wait(&ctl->bt_full[tb], tphase);
+    const uint32_t b_lo = desc_lo(bt_base + tb * kBt);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {   // K-major SW128: advancing K by 8 fp32 = +32 B inside the swizzle atom
+      wgmma_rs<NT>(acc[0], cur[kk], desc_of(b_lo + 2 * kk));
+      wgmma_rs<NT>(acc[1], cur[4 + kk], desc_of(b_lo + 2 * kk));
+    }
+    wgmma_commit();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&ctl->empty[stage]);   // this block's dY was loaded into registers (and X transposed)
+    if (++stage == p.stages) { stage = 0; phase ^= 1; }
+    // the previous block's wgmmas are done: its Bt buffer and its fragment registers (nxt) are free
+    if constexpr (kDouble) wgmma_wait<1>(); else wgmma_wait<0>();
+    if (pending && lane == 0) mbar_arrive(&ctl->bt_empty[tb ^ 1]);
+    pending = true;
+    tb ^= 1;
+    if (tb == 0) tphase ^= 1;
+    if (more) {
+      mbar_wait(&ctl->full[stage], phase);
+      load_a(nxt, stage_base + stage * stage_bytes);
+    }
+  };
+  for (int item = blockIdx.x; item < items; item += gridDim.x) {
+    const int tap = item / p.ksplits, ks = item % p.ksplits;
+    const int blk0 = static_cast<int>((static_cast<long long>(p.px_blocks) * ks) / p.ksplits);
+    const int blk1 = static_cast<int>((static_cast<long long>(p.px_blocks) * (ks + 1)) / p.ksplits);
+#pragma unroll
+    for (int i = 0; i < NT / 2; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
+    if (blk0 < blk1) {
+      mbar_wait(&ctl->full[stage], phase);
+      load_a(fa, stage_base + stage * stage_bytes);
+    }
+    for (int blk = blk0; blk < blk1; blk += 2) {
+      step(fa, kDouble ? fb : fa, blk + 1 < blk1);
+      if (blk + 1 == blk1) break;
+      step(kDouble ? fb : fa, fa, blk + 2 < blk1);
+    }
+    wgmma_wait<0>();
+    if (pending && lane == 0) mbar_arrive(&ctl->bt_empty[tb ^ 1]);
+    pending = false;
+    float* dst = p.partial + (static_cast<size_t>(ks) * taps + tap) * 128 * NT;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int j = 0; j < NT / 8; ++j) {
+        const int col = 8 * j + 2 * t;
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const int n = 64 * h + 16 * w + g + 8 * rr;   // output channel
+          *reinterpret_cast<float2*>(dst + static_cast<size_t>(n) * NT + col) =
+              make_float2(acc[h][4 * j + 2 * rr], acc[h][4 * j + 2 * rr + 1]);
+        }
+      }
+    }
+  }
+}
+
+// The bf16 weight gradient: the consumer warpgroup transposes the pixel-major stage (dY: 128 channels, X: NT channels,
+// kWgradKp pixels each, 128-byte swizzled rows of 64 bf16 channels) into K-major swizzled tiles At [128 rows][kWgradKp pixels]
+// and Bt [NT rows][kWgradKp pixels] (pixel pairs packed into 32-bit words), then D[n][c] += At * Bt^T.
+template <int NT>
+__device__ __forceinline__ void tc_wgrad_consumer_bf16(const TcWgradParams& p, SmemCtlW* ctl, uint8_t* smem, int stage_bytes,
+                                                       uint8_t* tbase, int items) {
+  constexpr int KE = 64;                             // channels per 128-byte source row
+  constexpr int E = 2;                               // bytes per element
   constexpr int kTA = kTileM * 128;                  // At: 128 rows of 128 bytes
-  constexpr int kTBuf = kTA + ((NT * 128 + 1023) & ~1023);
+  constexpr int kTBuf = wgrad_tbuf_bytes(true, NT);
   constexpr int kRows = 128 + NT;
   const int et = threadIdx.x - 128;
   const int w = et >> 5, lane = et & 31;
   constexpr int chunk_bytes = kWgradKp * 128;
   constexpr int y_bytes = (128 / KE) * chunk_bytes;
   constexpr int groups = kWgradKp * E / 16;          // 16-byte K groups per transposed row
-  constexpr int nk = kWgradKp / (BF16 ? 16 : 8);     // wgmma K steps per pixel block
+  constexpr int nk = kWgradKp / 16;                  // wgmma K steps per pixel block
   const int taps = p.kh * p.kw;
   int stage = 0, tb = 0;
   uint32_t phase = 0;
@@ -328,15 +511,10 @@ __device__ __forceinline__ void tc_wgrad_consumer(const TcWgradParams& p, SmemCt
         uint32_t v[4];
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
-          if (BF16) {
-            const int px = g * 8 + 2 * u;
-            const uint32_t lo = *reinterpret_cast<const uint16_t*>(src + px * 128 + ((((cb >> 4) ^ (px & 7)) << 4) | (cb & 15)));
-            const uint32_t hi = *reinterpret_cast<const uint16_t*>(src + (px + 1) * 128 + ((((cb >> 4) ^ ((px + 1) & 7)) << 4) | (cb & 15)));
-            v[u] = lo | (hi << 16);
-          } else {
-            const int px = g * 4 + u;
-            v[u] = *reinterpret_cast<const uint32_t*>(src + px * 128 + ((((cb >> 4) ^ (px & 7)) << 4) | (cb & 15)));
-          }
+          const int px = g * 8 + 2 * u;
+          const uint32_t lo = *reinterpret_cast<const uint16_t*>(src + px * 128 + ((((cb >> 4) ^ (px & 7)) << 4) | (cb & 15)));
+          const uint32_t hi = *reinterpret_cast<const uint16_t*>(src + (px + 1) * 128 + ((((cb >> 4) ^ ((px + 1) & 7)) << 4) | (cb & 15)));
+          v[u] = lo | (hi << 16);
         }
         uint8_t* dst = (is_y ? ta : tbb) + rs * 128 + ((g ^ (rs & 7)) << 4);
         *reinterpret_cast<uint4*>(dst) = make_uint4(v[0], v[1], v[2], v[3]);
@@ -348,8 +526,8 @@ __device__ __forceinline__ void tc_wgrad_consumer(const TcWgradParams& p, SmemCt
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < nk; ++k) {
-        wgmma_ss<NT, BF16>(acc[0], desc_of(a_lo + 2 * k), desc_of(b_lo + 2 * k));
-        wgmma_ss<NT, BF16>(acc[1], desc_of(a_lo + ((64u * 128u) >> 4) + 2 * k), desc_of(b_lo + 2 * k));
+        wgmma_ss<NT, true>(acc[0], desc_of(a_lo + 2 * k), desc_of(b_lo + 2 * k));
+        wgmma_ss<NT, true>(acc[1], desc_of(a_lo + ((64u * 128u) >> 4) + 2 * k), desc_of(b_lo + 2 * k));
       }
       wgmma_commit();
       wgmma_wait<1>();
@@ -374,6 +552,17 @@ __device__ __forceinline__ void tc_wgrad_consumer(const TcWgradParams& p, SmemCt
   }
 }
 
+template <bool DEEP, bool BF16, int NT>
+__device__ __forceinline__ void tc_wgrad_role(const TcWgradParams& p, SmemCtlW* ctl, uint8_t* smem, int stage_bytes,
+                                              uint8_t* tbase, int items, int warp) {
+  if constexpr (BF16) {
+    if (warp >= 4) tc_wgrad_consumer_bf16<NT>(p, ctl, smem, stage_bytes, tbase, items);
+  } else {
+    if (warp >= 4) tc_wgrad_mma<NT, !DEEP>(p, ctl, smem_u32(smem), stage_bytes, smem_u32(tbase), items);
+    else tc_wgrad_transposer<NT>(p, ctl, smem_u32(smem), stage_bytes, smem_u32(tbase), items);
+  }
+}
+
 template <bool DEEP, bool BF16 = false>
 __device__ __forceinline__ void tc_wgrad_body(const TcWgradParams& p, const TcWgradParams* pm, uint8_t* smem_raw) {
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -381,11 +570,10 @@ __device__ __forceinline__ void tc_wgrad_body(const TcWgradParams& p, const TcWg
   constexpr int YCH = 128 / KE;                                // chunks of dY (128 channels)
   constexpr int chunk_bytes = kWgradKp * 128;                  // kWgradKp pixel rows x KE channels
   const int y_bytes = YCH * chunk_bytes;                       // dY: 128 channels
-  const int x_bytes = p.c_chunks * chunk_bytes;                // X : c_pad channels
+  const int x_bytes = p.c_chunks * chunk_bytes;                // X : c_chunks * KE channels
   const int stage_bytes = y_bytes + x_bytes;
   uint8_t* tbase = smem + p.stages * stage_bytes;              // two transposed operand buffers
-  const int tbuf = kTileM * 128 + round1024(p.n_cols * 128);
-  SmemCtlW* ctl = reinterpret_cast<SmemCtlW*>(tbase + 2 * tbuf);
+  SmemCtlW* ctl = reinterpret_cast<SmemCtlW*>(tbase + 2 * wgrad_tbuf_bytes(BF16, p.n_cols));
   const int items = p.kh * p.kw * p.ksplits;
 
   const int warp = threadIdx.x >> 5;
@@ -398,7 +586,11 @@ __device__ __forceinline__ void tc_wgrad_body(const TcWgradParams& p, const TcWg
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < p.stages; ++i) {
       mbar_init(&ctl->full[i], 1);
-      mbar_init(&ctl->empty[i], 4);   // one arrival per consumer warp
+      mbar_init(&ctl->empty[i], BF16 ? 4 : 7);   // one arrival per consumer warp (tf32: and per transposer warp)
+    }
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(&ctl->bt_full[i], 96);   // every transposer thread
+      mbar_init(&ctl->bt_empty[i], 4);   // one arrival per MMA warp
     }
     fence_mbar_init();
   }
@@ -435,13 +627,14 @@ __device__ __forceinline__ void tc_wgrad_body(const TcWgradParams& p, const TcWg
         if (++stage == p.stages) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp >= 4) {
+  } else {
     switch (p.n_cols) {
-      case 32: tc_wgrad_consumer<BF16, 32>(p, ctl, smem, stage_bytes, tbase, items); break;
-      case 64: tc_wgrad_consumer<BF16, 64>(p, ctl, smem, stage_bytes, tbase, items); break;
-      case 96: tc_wgrad_consumer<BF16, 96>(p, ctl, smem, stage_bytes, tbase, items); break;
-      case 128: tc_wgrad_consumer<BF16, 128>(p, ctl, smem, stage_bytes, tbase, items); break;
-      default: tc_wgrad_consumer<BF16, 160>(p, ctl, smem, stage_bytes, tbase, items); break;
+      case 32: tc_wgrad_role<DEEP, BF16, 32>(p, ctl, smem, stage_bytes, tbase, items, warp); break;
+      case 64: tc_wgrad_role<DEEP, BF16, 64>(p, ctl, smem, stage_bytes, tbase, items, warp); break;
+      case 96: tc_wgrad_role<DEEP, BF16, 96>(p, ctl, smem, stage_bytes, tbase, items, warp); break;
+      case 128: tc_wgrad_role<DEEP, BF16, 128>(p, ctl, smem, stage_bytes, tbase, items, warp); break;
+      case 136: tc_wgrad_role<DEEP, BF16, 136>(p, ctl, smem, stage_bytes, tbase, items, warp); break;
+      default: tc_wgrad_role<DEEP, BF16, 160>(p, ctl, smem, stage_bytes, tbase, items, warp); break;
     }
   }
   __syncthreads();
@@ -464,7 +657,7 @@ size_t tc_conv_smem_bytes(const TcConvParams& p) {
 }
 size_t tc_wgrad_smem_bytes(const TcWgradParams& p) {
   const size_t chunk = static_cast<size_t>(kWgradKp) * 128;
-  const size_t tbuf = kTileM * 128 + round1024(p.n_cols * 128);
+  const size_t tbuf = wgrad_tbuf_bytes(p.bf16 != 0, p.n_cols);
   return 1024 + p.stages * ((p.bf16 ? 2 : 4) * chunk + static_cast<size_t>(p.c_chunks) * chunk) + 2 * tbuf + sizeof(SmemCtlW);
 }
 
@@ -505,8 +698,9 @@ int tc_conv_grid(const TcConvParams& p, int num_sms) {
 
 cudaError_t tc_wgrad_launch(const TcWgradParams& p, cudaStream_t s) {
   const size_t smem = tc_wgrad_smem_bytes(p);
-  if (smem > kMaxSmem || p.n_cols % 32 != 0 || p.n_cols < 32 || p.n_cols > 160 ||
-      p.stages < 1 || p.stages > 8)
+  const bool cols_ok = p.n_cols == 32 || p.n_cols == 64 || p.n_cols == 96 || p.n_cols == 128 || p.n_cols == 136 ||
+                       p.n_cols == 160;
+  if (smem > kMaxSmem || !cols_ok || p.n_cols > p.c_chunks * (p.bf16 ? 64 : 32) || p.stages < 1 || p.stages > 8)
     return cudaErrorInvalidValue;
   return launch_k(p.bf16 ? tc_wgrad_kernel_bf16 : tc_wgrad_kernel, dim3(p.kh * p.kw * p.ksplits), dim3(kNumThreads), smem, s, 1, p);
 }

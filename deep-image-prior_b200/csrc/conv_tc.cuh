@@ -46,7 +46,7 @@ struct TcConvParams {
 //   dY : NHWC [H][W][N] (fp32 or bf16 twin; N <= 128 output channels, channels >= N read as zero) through a 3-D map (N, W, H)
 //   X  : conv input through the same 5-D view as in TcConvParams
 //   A work item is one filter tap and one split-K range of pixel blocks (kh * kw * ksplits items); it writes its own
-//   slice of partials [ksplit][tap][128][c_pad], which a follow-up kernel sums in a fixed order -- the gradient does not
+//   slice of partials [ksplit][tap][128][n_cols], which a follow-up kernel sums in a fixed order -- the gradient does not
 //   depend on the order in which work items finish (fp32 atomics here made runs drift apart over thousands of steps).
 // pixels per K block of the weight-gradient GEMM (TMA box width; one transposed 128-byte row holds 32 fp32 pixels).  A row
 // shorter than a multiple of 32 reads zero-filled dY past its end, which adds nothing.
@@ -54,13 +54,14 @@ static constexpr int kWgradKp = 32;
 struct TcWgradParams {
   CUtensorMap tmY;
   CUtensorMap tmX;
-  float* partial;          // [ksplits][kh*kw][128][c_pad], every element written by the kernel
+  float* partial;          // [ksplits][kh*kw][128][n_cols], every element written by the kernel
   int kh, kw, stride, offx, offy;
   int px_blocks_x;         // ceil(W / kWgradKp)
   int px_blocks;           // total pixel blocks = H * px_blocks_x
   int bf16;                // 1: dY / X are bf16 (chunks of 64 channels, K = 16 pixels per wgmma)
   int c_chunks;            // 128-byte channel chunks of X (32 fp32 / 64 bf16 channels each)
-  int n_cols;              // wgmma N = accumulator columns per tap = row stride of `partial` (multiple of 32, <= 160)
+  int n_cols;              // wgmma N = accumulator columns per tap = row stride of `partial`: 32, 64, 96, 128, 136 or 160
+                           // (<= the channels of the X chunks; channels past C are zero in X, so their columns are zero)
   int ksplits;             // work items per filter tap
   int stages;
 };

@@ -204,7 +204,7 @@ struct ConvOp {
   float* out = nullptr; int out_h = 0, out_w = 0;
   double* stats = nullptr;
   float* wp_f = nullptr; float* wp_d = nullptr;
-  float* wacc = nullptr;   // plan-owned weight-gradient partials [ksplits][tap][128][c_pad] (tensor-core path)
+  float* wacc = nullptr;   // plan-owned weight-gradient partials [ksplits][tap][128][wg_cols()] (tensor-core path)
   // dgrad: dg_in [dg_in_h][dg_in_w][128] -> dg_out [dg_out_h][dg_out_w][C]
   bool has_dgrad = false;
   bool dg_s2 = false;   // tensor-core dgrad of a stride-2 3x3 conv as its 4 sub-pixel phases (dg_in = dY [h][w][128], not zero-stuffed)
@@ -228,8 +228,11 @@ struct ConvOp {
   }
   size_t wp_f_elems() const { return (size_t)k * k * Np * c_pad; }
   size_t wp_d_elems() const { return (size_t)k * k * crows * n_pad; }
-  size_t wacc_elems() const { return (size_t)tc_ksplits() * k * k * 128 * c_pad; }
-  // work items per filter tap: about one item per SM of an H100 SXM over all taps (every item writes a [128][c_pad] partial
+  size_t wacc_elems() const { return (size_t)tc_ksplits() * k * k * 128 * wg_cols(); }
+  // accumulator columns of the tensor-core weight gradient (wgmma N, row stride of its partials): c_pad, except 136 for
+  // 128 < C <= 136 (the 128 + 4 channel concat convs), which would otherwise multiply 24 zero columns of every 160
+  int wg_cols() const { return C > 128 && C <= 136 ? 136 : c_pad; }
+  // work items per filter tap: about one item per SM of an H100 SXM over all taps (every item writes a [128][wg_cols] partial
   // slice, so more items than SMs only add traffic).  A constant, not the device's count: the plan's size is known
   // without a device, and the split -- hence the summation order of the gradient -- is the same on every device.
   int tc_ksplits() const {
@@ -323,7 +326,7 @@ struct ConvOp {
     wg.px_blocks_x = (wg_w + kWgradKp - 1) / kWgradKp;
     wg.px_blocks = wg_h * wg.px_blocks_x;
     wg.c_chunks = bf16 ? c_pad16 / 64 : c_pad / 32;
-    wg.n_cols = c_pad;
+    wg.n_cols = wg_cols();
     wg.ksplits = tc_ksplits();
     wg.stages = 6;
     while (tc_wgrad_smem_bytes(wg) > 232448 && wg.stages > 1) wg.stages--;
@@ -378,7 +381,7 @@ struct ConvOp {
         DIP_CUDA(tc_wgrad_launch(p, s));
       }
       if (wacc != nullptr) return 0;
-      launch_wgrad_reduce(partial, p.ksplits, N, C, k, k, rot, c_pad, dw, s, Ctot, coff);
+      launch_wgrad_reduce(partial, p.ksplits, N, C, k, k, rot, p.n_cols, dw, s, Ctot, coff);
       DIP_CUDA(cudaGetLastError());
       return 0;
     } else {
@@ -438,11 +441,11 @@ __global__ void k_pack_table(const PackEntry* __restrict__ tab) {
     }
   }
 }
-// partials [ks][tap][128][c_pad] of all tensor-core weight gradients -> OIHW gradients (one launch per backward pass);
+// partials [ks][tap][128][cols] of all tensor-core weight gradients -> OIHW gradients (one launch per backward pass);
 // the split-K slices are summed in index order, so the gradient is the same on every run
 struct UnpackEntry {
   const float* acc; float* dw;
-  int N, C, taps, rot, c_pad, Ctot, coff, ks;
+  int N, C, taps, rot, cols, Ctot, coff, ks;   // cols: row stride of the partials (ConvOp::wg_cols)
 };
 __global__ void k_wgrad_unpack_table(const UnpackEntry* __restrict__ tab) {
   pdl_enter();
@@ -450,8 +453,8 @@ __global__ void k_wgrad_unpack_table(const UnpackEntry* __restrict__ tab) {
   const int total = e.N * e.C * e.taps;   // dw elements this entry owns: (n, engine channel c, tap)
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     const int tap = i % e.taps, c = (i / e.taps) % e.C, n = i / (e.taps * e.C);
-    const size_t split = (size_t)e.taps * 128 * e.c_pad;
-    const float* src = e.acc + ((size_t)tap * 128 + n) * e.c_pad + c;
+    const size_t split = (size_t)e.taps * 128 * e.cols;
+    const float* src = e.acc + ((size_t)tap * 128 + n) * e.cols + c;
     float v = 0.f;
     for (int k = 0; k < e.ks; ++k) v += src[k * split];
     e.dw[((size_t)n * e.Ctot + (c + e.coff + e.rot) % e.Ctot) * e.taps + tap] = v;
@@ -1015,7 +1018,7 @@ static int upload_tables(dip_plan* P) {
     std::vector<UnpackEntry> up;
     for (ConvOp* op : P->convs) {
       if (!op->do_wgrad || op->wacc == nullptr) continue;
-      up.push_back(UnpackEntry{op->wacc, P->grads[op->p_w], op->N, op->C, op->k * op->k, op->rot, op->c_pad, op->Ctot, op->coff,
+      up.push_back(UnpackEntry{op->wacc, P->grads[op->p_w], op->N, op->C, op->k * op->k, op->rot, op->wg_cols(), op->Ctot, op->coff,
                                op->wg.ksplits});
     }
     if ((int)up.size() != P->n_unpack) return fail("internal: unpack table size mismatch");

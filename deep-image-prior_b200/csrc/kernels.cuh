@@ -227,6 +227,7 @@ void launch_pack_fprop(const float* w, int N, int C, int kh, int kw, int rot, fl
 void launch_pack_dgrad(const float* w, int N, int C, int kh, int kw, int rot, float* dst, int c_rows, int n_pad,
                        cudaStream_t s);
 // split-K partials [ksplits][tap][128][c_pad] -> OIHW gradient [N][C][kh][kw]
+//   c_pad: row stride of the partials (a multiple of 4, >= C; the tensor-core path passes its accumulator columns)
 //   dw has Ctot input channels; the partials cover engine channels [coff, coff + C): torch channel (c + coff + rot) % Ctot
 //   (Ctot = 0: Ctot = C)
 void launch_wgrad_reduce(const float* partial, int ksplits, int N, int C, int kh, int kw, int rot, int c_pad,
