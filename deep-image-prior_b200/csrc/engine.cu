@@ -853,17 +853,21 @@ static int build_plan(dip_plan* P, Arena& A) {
       reg(pf + "dRaw_v16", v.dRaw_v16, v.H, v.W, nu, nu);
       reg(pf + "dRaw_u16", v.dRaw_u16, v.H, v.W, nu, nu);
       reg(pf + "dRaw_d2_16", v.dRaw_d2_16, v.h, v.w, nd, nd);
-      reg(pf + "dRaw_d1_16", v.dRaw_d1_16, v.h, v.w, nd, nd);
+      if (!avg) reg(pf + "dRaw_d1_16", v.dRaw_d1_16, v.h, v.w, nd, nd);   // (avg: the pooled gradient stays fp32)
       if (wide) reg(pf + "dRaw_s16", v.dRaw_s16, v.H, v.W, 128, 128);
     }
-    if (l > 0) {
-      reg(pf + "ZS", v.ZS, v.H, v.W, nd, nd);
-      reg(pf + "dPin", v.dPin, v.H + 2, v.W + 2, v.Cin, v.Cin);
+    reg(pf + "dUp", v.dUp, v.h, v.w, v.cu, v.cu);
+    if (avg) {
+      reg(pf + "rawF", v.rawF, v.H, v.W, nd, nd);
+      if (bf) reg(pf + "dRawF16", v.dRawF16, v.H, v.W, nd, nd);   // bf16 mode writes the conv's dY as the twin only
+      else reg(pf + "dRawF", v.dRawF, v.H, v.W, nd, nd);
     }
+    if (v.dS != nullptr && CS > 0) reg(pf + "dS", v.dS, v.H, v.W, v.Cin, v.Cin);   // (written by the skip conv's dgrad only)
+    if (v.ZS != nullptr) reg(pf + "ZS", v.ZS, v.H, v.W, nd, nd);
+    if (v.dPin != nullptr) reg(pf + "dPin", v.dPin, v.H + 2, v.W + 2, v.Cin, v.Cin);
   }
   P->out_saved = A.get<float>((size_t)P->H * P->W * d.out_channels);
   P->zbuf = A.get<float>((size_t)P->H * P->W * d.in_channels);
-  reg("zbuf", P->zbuf, d.in_channels, P->H, P->W, P->W);   // torch-layout planes [C][H][W]: the runner's perturbed input
   P->dout = A.get<float>((size_t)P->H * P->W * d.out_channels);
   P->dl4 = A.get<float>((size_t)P->H * P->W * 4);
   P->ds_kern = A.get<float>(dip_plan::kDownMaxK * dip_plan::kDownMaxK);
@@ -1404,7 +1408,7 @@ static DeepOp deep_bn_act_write(dip_plan* P, const float* raw, const BnLayer& b,
 }
 static void deep_fwd_level(dip_plan* P, int l, std::vector<DeepOp>& ops) {
   Level& v = P->lv[l];
-  const int CS = P->desc.skip_channels;
+  const int CS = v.ns;
   const bool last = l == (int)P->lv.size() - 1;
   const float* pin_interior = v.Pin + ((size_t)(v.W + 2) + 1) * v.Cin;
   // skip branch (independent of the deeper branch until the concat: no barrier behind it)
@@ -1425,7 +1429,7 @@ static void deep_fwd_level(dip_plan* P, int l, std::vector<DeepOp>& ops) {
   {
     DeepOp o;
     o.type = DO_CAT_STATS;
-    vec_lanes(128 + CS, &o.VL, &o.PPB);
+    vec_lanes(v.cu + CS, &o.VL, &o.PPB);
     o.u.cat = DeepCat{cat_args(P, v, level_usrc(P, l)), v.bn_cat.fwd, bn_ref(P, v.bn_cat), v.P_cat};
     ops.push_back(o);
     o.type = DO_CAT_WRITE;
@@ -1459,7 +1463,7 @@ static DeepOp deep_wgrad(dip_plan* P, const ConvOp& op, int sync = 1) {
 }
 static void deep_bwd_level(dip_plan* P, int l, GradSrc src_v, std::vector<DeepOp>& ops) {
   Level& v = P->lv[l];
-  const int CS = P->desc.skip_channels, CC = 128 + CS;
+  const int CS = v.ns, CC = v.cu + v.ns;
   const bool last = l == (int)P->lv.size() - 1;
   // 1x1 conv + BN + LReLU
   deep_bn_bwd(P, v.raw_v, 128, v.bn_v, src_v, v.H, v.W, v.dRaw_v, ops);
@@ -1528,8 +1532,10 @@ static int build_deep_ops(dip_plan* P) {
   P->n_deep_fwd = P->n_deep_bwd = 0;
   P->deep_grid = 128 < g_num_sms ? 128 : g_num_sms;
   if (P->desc.precision != DIP_PRECISION_TF32 || (int)P->lv.size() <= P->deep_from) return 0;
-  for (const Level& v : P->lv)   // the op lists below are written for the 128-wide network with a skip branch at every scale
-    if (v.nd != 128 || v.nu != 128 || v.ns == 0 || v.ns != P->lv[0].ns) return 0;
+  // the op lists below are written for the 128-wide stride-2 network with the same skip branch (4 or 128 channels) at
+  // every scale: they have no pooling pass (downsample_mode 'avg' normalises the pooled raw_d1, which only fwd_level writes)
+  for (const Level& v : P->lv)
+    if (v.nd != 128 || v.nu != 128 || v.ns == 0 || v.ns != P->lv[0].ns || v.rawF != nullptr) return 0;
   std::vector<DeepOp> fwd;
   deep_fwd_level(P, P->deep_from, fwd);
   if ((int)fwd.size() > dip_plan::kDeepMaxOps) return fail("internal: deep forward op list too long");

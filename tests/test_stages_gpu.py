@@ -1,0 +1,310 @@
+"""P1 stage tier: one forward + backward on the GPU, then every stage of the step checked on its own (teacher forcing).
+
+Each stage's reference (tests/stage_ref.py) is computed in fp64 on the GPU from the engine's own input buffers of that
+stage, so no error carries over from earlier stages and no LeakyReLU branch flips: the tolerance is the rounding of that
+one stage, element by element (convolutions: 2 (e_op + n 2^-23) M; memory-bound stages: 1e-5 |ref| + 3e-5 s_c; see the
+module docstring of stage_ref.py).  Parameters are away from init (random gamma, beta and biases, different for the
+skip and up channels of every concat BN), and every registered buffer is filled with NaN before the first pass, so a
+halo cell, tail or tile edge that no kernel writes shows up as a non-finite stage output.
+"""
+import ctypes
+import os
+
+import pytest
+import torch
+
+from oracle import dip_oracle as O
+import stage_ref as SR
+
+pytestmark = pytest.mark.gpu
+MODES = ["fp32", "tf32", "bf16"]
+LEVEL_BUFFERS = ["Pin", "raw_s", "raw_d1", "rawF", "P_d1", "raw_d2", "P_d2", "P_cat", "raw_u", "A_u", "raw_v", "U",
+                 "dRaw_v", "dA_u", "dRaw_u", "dP_cat", "dCat", "dRaw_s", "dUp", "dS", "dRaw_d2", "dP_d1", "dRaw_d1",
+                 "dRawF", "dPin", "Pin16", "P_d1_16", "P_d2_16", "P_cat16", "A_u16", "dRaw_v16", "dRaw_u16", "dRaw_d2_16",
+                 "dRaw_d1_16", "dRaw_s16", "dRawF16"]
+# (not "ZS": the zero-stuffed dY of the exact-fp32 stride-2 input gradient.  The BN backward writes its even positions
+# only (d_bn_bwd_apply in kernels_mem.cu, the `zs` store), and the odd ones keep the zeros that build_plan writes once
+# when dip_plan_create builds the plan: the cudaMemset of every level's ZS after "The zero-stuffed buffers are written
+# at even positions only: clear them once" in engine.cu.)
+WORST = {}   # mode -> {stage: worst |err| / tolerance}
+FROB = {}    # mode -> {conv stage: worst relative Frobenius error / its bound}
+
+
+def cfg_of(kind):
+    c = {
+        "cs4": lambda: O.SkipConfig(skip_channels=4, upsample_mode="bilinear"),
+        "cs128": lambda: O.SkipConfig(skip_channels=128, upsample_mode="nearest"),
+        "cs0": lambda: O.SkipConfig(skip_channels=0, upsample_mode="bilinear"),
+        "snail": lambda: O.SkipConfig(in_channels=3, channels=[8, 16, 32, 64, 128], skip_channels=[0, 0, 0, 4, 4]),
+        "kate": lambda: O.SkipConfig(in_channels=3, channels=[16, 32, 64, 128, 128], skip_channels=0),
+        "modes": lambda: O.SkipConfig(in_channels=3, skip_channels=4,
+                                      upsample_mode=["bilinear", "nearest", "bilinear", "nearest", "nearest"]),
+        "ingrad": lambda: O.SkipConfig(skip_channels=4, out_channels=1, need_sigmoid=False),
+        "per_scale128": lambda: O.SkipConfig(channels=[128] * 5, skip_channels=[4] * 5),
+        "avg128": lambda: O.SkipConfig(skip_channels=4),
+    }[kind]()
+    if kind in ("kate", "avg128"):
+        c.downsample_mode = "avg"
+    return c
+
+
+def make_plan(cfg, H, W, mode, input_grad=False):
+    import dip_engine as de
+    prec = {"fp32": de.PRECISION_FP32, "tf32": de.PRECISION_TF32, "bf16": de.PRECISION_BF16}[mode]
+    bil = cfg.upsample_mode == "bilinear" if isinstance(cfg.upsample_mode, str) else [m == "bilinear" for m in cfg.upsample_mode]
+    L = cfg.num_scales
+    per_scale = isinstance(cfg.channels, (list, tuple)) or isinstance(cfg.skip_channels, (list, tuple))
+    ch = [cfg.nd(l) for l in range(L)] if per_scale else cfg.channels
+    sk = [cfg.ns(l) for l in range(L)] if per_scale else cfg.skip_channels
+    return de.Plan(cfg.in_channels, cfg.out_channels, L, ch, sk, bil, H, W, precision=prec, need_sigmoid=cfg.need_sigmoid,
+                   input_grad=input_grad, downsample_mode=cfg.downsample_mode)
+
+
+def buffer_view(plan, name):
+    """the registered buffer's [:, :, :c] region inside the workspace (a view; Plan.buffer returns a copy), or None"""
+    import dip_engine as de
+    p = ctypes.c_void_p()
+    dims = (ctypes.c_int * 4)()
+    if de.lib().dip_plan_buffer(plan.h, name.encode(), ctypes.byref(p), dims) != 0:
+        return None
+    rows, cols, ld, c = dims[0], dims[1], dims[2], dims[3]
+    esz = 2 if name.endswith("16") else 4
+    off = p.value - plan.workspace.data_ptr()
+    flat = plan.workspace[off:off + rows * cols * ld * esz].view(torch.bfloat16 if esz == 2 else torch.float32)
+    return flat.view(rows, cols, ld)[:, :, :c]
+
+
+def fill_nan(plan, L):
+    n = 0
+    for l in range(L):
+        for b in LEVEL_BUFFERS:
+            v = buffer_view(plan, "L%d.%s" % (l, b))
+            if v is not None and v.numel():
+                v.fill_(float("nan"))
+                n += 1
+    torch.cuda.synchronize()
+    assert n > 0
+
+
+def fp32_dropped(cfg, name):
+    """bf16 mode keeps only the bf16 twin of these stage outputs (DESIGN.md section 2; engine.cu fwd_level / bn_bwd)"""
+    l, b = int(name[1]), name.split(".", 1)[1]
+    if b in ("P_d1", "A_u", "dRaw_v", "dRaw_u", "dRaw_d2", "dRawF"):
+        return True
+    if b == "dRaw_d1":
+        return cfg.downsample_mode != "avg"
+    if b == "dRaw_s":
+        return cfg.ns(l) == 128
+    if b == "P_d2":
+        return l < cfg.num_scales - 1 and cfg.ns(l + 1) != 4
+    return False
+
+
+def bf16_ulp(x):
+    a = x.abs().clamp_min(2.0 ** -126)
+    return torch.exp2(torch.floor(torch.log2(a)) - 7)
+
+
+def ratio_of(got, ref, tol, excl):
+    d = (got.double() - ref).abs()
+    r = torch.where(d == 0, torch.zeros_like(d), d / tol.expand_as(d))
+    if excl is not None:
+        r = torch.where(excl, torch.zeros_like(r), r)
+    return r
+
+
+def check(tag, cfg, mode, plan, refs, dgrads, out, dz=None):
+    names = [n for n, _ in O.param_layout(cfg)]
+    table = WORST.setdefault(mode, {})
+    failures = []
+    for name, (ref, tol, excl) in refs.d.items():
+        if name.startswith("grad:"):
+            got = dgrads[names.index(name[5:])].double()
+        elif name == "out":
+            got = out[0].double()
+        elif name == "dz":
+            got = dz.double()
+        elif mode == "bf16" and fp32_dropped(cfg, name):
+            got = None
+        else:
+            got = plan.buffer(name).double()
+        if mode == "bf16" and not name.startswith("grad:") and name not in ("out", "dz"):
+            twin = buffer_view(plan, SR._twin(name))
+            if twin is not None:
+                twin = twin.double()
+                if got is not None:   # the twin of a kept fp32 tensor is its round-to-nearest-even copy
+                    if not torch.equal(twin, SR.bf16(got)):
+                        failures.append("%s: bf16 twin != bf16(fp32 tensor)" % name)
+                else:                 # only the twin exists: one bf16 ulp of the rounded reference, few elements differ
+                    rb = SR.bf16(ref)
+                    d = (twin - rb).abs()
+                    bad = d > bf16_ulp(rb) + 2 * tol
+                    if excl is not None:
+                        bad &= ~excl
+                    if not torch.isfinite(twin).all() or bad.any() or (d > 0).sum().item() > 1e-2 * d.numel() + 8:
+                        failures.append("%s (bf16 twin): %d elements beyond one ulp, %d differ of %d" % (
+                            name, bad.sum().item(), (d > 0).sum().item(), d.numel()))
+                    continue
+        if got is None:   # a stage that bf16 mode keeps as a twin only, but whose twin is not registered: unchecked
+            failures.append("%s: fp32 tensor dropped in bf16 mode, but no bf16 twin %s is registered" % (name, SR._twin(name)))
+            continue
+        if not torch.isfinite(got).all():
+            idx = (~torch.isfinite(got)).nonzero()[0].tolist()
+            failures.append("%s: %d non-finite elements (unwritten memory?), first at %s" % (
+                name, (~torch.isfinite(got)).sum().item(), idx))
+            continue
+        r = ratio_of(got, ref, tol, excl)
+        worst = r.max().item()
+        key = name.split(".", 1)[1] if name.startswith("L") else name
+        key = "grad:" + name.split(".", 1)[1] if name.startswith("grad:L") else key
+        table[key] = max(table.get(key, 0.0), worst)
+        if name in refs.conv:   # convolutions: relative Frobenius error at the precision the kernel runs in
+            bound = SR.FROB_TOL[refs.conv[name]]
+            dn, rn = (got - ref).norm().item(), ref.norm().item()
+            fro = dn / rn if rn > 0 else (0.0 if dn == 0 else float("inf"))
+            ftab = FROB.setdefault(mode, {})
+            ftab[key] = max(ftab.get(key, (0.0, 0.0)), (fro / bound, fro))
+            if not fro <= bound:
+                failures.append("%s: relative Frobenius error %.3g > %.1g (%s kernel)" % (name, fro, bound, refs.conv[name]))
+        if not worst <= 1.0:
+            i = tuple(torch.unravel_index(r.argmax(), r.shape))
+            i = tuple(int(x) for x in i)
+            failures.append("%s: worst |err|/tol = %.3g at %s (got %.9g ref %.9g tol %.3g)" % (
+                name, worst, i, got[i].item(), ref[i].item(), tol.expand_as(r)[i].item()))
+    for name, (frac, n) in refs.excl.items():   # (one element may sit there in the 768 of a 2 x 3 x 128 map)
+        if frac >= 1e-3 + 1.5 / n:
+            failures.append("%s: %.2g of the elements sit at the LeakyReLU boundary" % (name, frac))
+    assert not failures, "[%s %s]\n  " % (tag, mode) + "\n  ".join(failures)
+
+
+def params_for(cfg, seed=0):
+    return [p.float() for p in SR.random_affine(cfg, O.init_params(cfg, seed=seed), seed=seed + 11)]
+
+
+def run_direct(cfg, H, W, mode, input_grad=False, seed=0):
+    """plan.forward / plan.backward with dout = the MSE gradient against a random target; every stage checked"""
+    params = params_for(cfg, seed)
+    g = torch.Generator().manual_seed(seed + 1)
+    z = torch.rand(1, cfg.in_channels, H, W, generator=g).cuda()
+    target = torch.rand(1, cfg.out_channels, H, W, generator=g).cuda()
+    plan = make_plan(cfg, H, W, mode, input_grad)
+    dparams = [p.cuda().contiguous() for p in params]
+    dgrads = [torch.zeros_like(p) for p in dparams]
+    plan.bind(dparams, dgrads)
+    fill_nan(plan, cfg.num_scales)
+    out = plan.forward(z)
+    dout = (2.0 * (out - target) / out.numel()).contiguous()
+    plan.backward(dout)
+    dz = plan.input_grad() if input_grad else None
+    torch.cuda.synchronize()
+    refs = SR.Refs()
+    src = plan.buffer if mode != "bf16" else (lambda n: buffer_view(plan, n) if n.endswith("16") else plan.buffer(n))
+    SR.forward(cfg, dparams, lambda n: out[0] if n == "out" else src(n), mode, refs, z=z)
+    SR.backward(cfg, dparams, lambda n: out[0] if n == "out" else src(n), mode, refs, dout[0], input_grad=input_grad)
+    check("%s %dx%d" % (cfg_tag(cfg), H, W), cfg, mode, plan, refs, dgrads, out, dz)
+    return plan
+
+
+def cfg_tag(cfg):
+    return "in%d out%d ch%s skip%s %s %s" % (cfg.in_channels, cfg.out_channels, cfg.channels, cfg.skip_channels,
+                                            cfg.upsample_mode, cfg.downsample_mode)
+
+
+def print_table():
+    for mode in MODES:
+        if mode in WORST:
+            row = sorted(WORST[mode].items())
+            print("\n[stage tier %s] worst |err|/tol per stage: %s" % (mode, ", ".join("%s %.2g" % kv for kv in row)))
+        if mode in FROB:
+            row = sorted(FROB[mode].items())
+            print("[stage tier %s] conv stages, worst relative Frobenius error (/ its bound): %s" % (
+                mode, ", ".join("%s %.2g (%.2g)" % (k, v[1], v[0]) for k, v in row)))
+
+
+CASES = [("cs4", 64, 96, False), ("cs128", 96, 64, False), ("cs0", 64, 96, False), ("snail", 64, 96, False),
+         ("kate", 96, 64, False), ("modes", 64, 96, False), ("ingrad", 64, 96, True), ("cs4", 256, 384, False)]
+
+
+@pytest.mark.parametrize("mode", MODES)
+@pytest.mark.parametrize("case", CASES, ids=["%s_%dx%d" % c[:3] for c in CASES])
+def test_every_stage_direct(case, mode):
+    kind, H, W, input_grad = case
+    run_direct(cfg_of(kind), H, W, mode, input_grad)
+    print_table()
+
+
+def test_every_stage_flagship_512_tf32():
+    run_direct(cfg_of("cs4"), 512, 512, "tf32")
+    print_table()
+
+
+def run_runner(cfg, H, W, mode, task):
+    """one iteration of the device runner (the path bench.py measures) at lr = 0: Adam leaves the parameters bitwise
+    unchanged, so the buffers describe one step at known parameters.  The loss / downsampler gradient is checked through
+    the L0.dRaw_v composite, from the output and the target; the noisy padded input is taken as given."""
+    import dip_engine as de
+    params = params_for(cfg, 3)
+    g = torch.Generator().manual_seed(5)
+    z0 = torch.rand(1, cfg.in_channels, H, W, generator=g).cuda()
+    plan = make_plan(cfg, H, W, mode)
+    mask = down = None
+    if task == "sr":
+        kern = O.down_kernel(4, "lanczos2", 0.5)
+        down = (torch.from_numpy(kern).double(), 4, O.down_pad(kern.shape[0], 4))
+        plan.set_downsampler(torch.from_numpy(kern).float(), 4, down[2])
+        th, tw = de.down_out_size(H, kern.shape[0], 4, down[2]), de.down_out_size(W, kern.shape[0], 4, down[2])
+    else:
+        th, tw = H, W
+    target = torch.rand(1, cfg.out_channels, th, tw, generator=g).cuda()
+    if task == "inpaint":
+        mask = (torch.rand(1, 1, H, W, generator=g) > 0.3).float().cuda()
+    dparams = [p.cuda().contiguous() for p in params]
+    dgrads = [torch.zeros_like(p) for p in dparams]
+    plan.bind(dparams, dgrads)
+    for p, gb in zip(dparams, dgrads):
+        p.grad = gb
+    adam = de.FusedAdam(dparams, lr=0.0)
+    adam._bind(dgrads)
+    before = [p.clone() for p in dparams]
+    fill_nan(plan, cfg.num_scales)
+    out = torch.empty(1, cfg.out_channels, H, W, device="cuda")
+    de.run_iterations(plan, adam, z0, target, mask, 1. / 30, 7, 1, 0.0, out=out)
+    torch.cuda.synchronize()
+    assert all(torch.equal(a, b) for a, b in zip(before, dparams))
+    o = out.double().cpu().requires_grad_(True)
+    lo = o if down is None else O.downsample(o, *down)
+    loss = O.mse_loss(lo, target.double().cpu(), None if mask is None else mask.double().cpu())
+    dout = torch.autograd.grad(loss, o)[0].cuda()
+    src = plan.buffer if mode != "bf16" else (lambda n: buffer_view(plan, n) if n.endswith("16") else plan.buffer(n))
+    rd = lambda n: out[0] if n == "out" else src(n)   # noqa: E731
+    refs = SR.Refs()
+    SR.forward(cfg, dparams, rd, mode, refs)
+    SR.backward(cfg, dparams, rd, mode, refs, dout[0])
+    check("runner %s %s %dx%d" % (task, cfg_tag(cfg), H, W), cfg, mode, plan, refs, dgrads, out)
+
+
+@pytest.mark.parametrize("task,kind,H,W,mode", [("denoise", "cs4", 128, 128, "tf32"), ("inpaint", "cs128", 128, 192, "tf32"),
+                                                 ("sr", "cs4", 256, 256, "tf32"), ("sr", "cs4", 256, 256, "bf16")])
+def test_every_stage_runner(task, kind, H, W, mode):
+    run_runner(cfg_of(kind), H, W, mode, task)
+    print_table()
+
+
+@pytest.mark.parametrize("kind,engages", [("cs4", True), ("cs128", True), ("avg128", False), ("per_scale128", True)])
+def test_every_stage_deep_kernel(kind, engages):
+    """DIP_DEEP=1 (levels >= 2 as one persistent kernel per pass): the same stage checks.  The deep op lists have no
+    pooling pass, so a downsample_mode='avg' network must keep the launch-by-launch path."""
+    cfg = cfg_of(kind)
+    H, W = (96, 64) if kind == "cs128" else (64, 96)
+    plan0 = run_direct(cfg, H, W, "tf32")
+    os.environ["DIP_DEEP"] = "1"
+    try:
+        plan = run_direct(cfg, H, W, "tf32")
+    finally:
+        os.environ.pop("DIP_DEEP", None)
+    (f0, b0), (f1, b1) = plan0.num_launches(), plan.num_launches()
+    if engages:
+        assert f1 < f0 - 20 and b1 < b0 - 40, ((f0, b0), (f1, b1))
+    else:
+        assert (f1, b1) == (f0, b0)
+    print_table()
