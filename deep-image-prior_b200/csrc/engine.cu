@@ -548,6 +548,7 @@ using namespace dip;
 struct dip_plan {
   dip_net_desc desc;
   int H, W;
+  int zero_pad = 0;   // dip_plan_opts.pad_mode == DIP_PAD_ZERO: conv-input halos hold zeros (Conv2d(padding=1))
   bool dry = false;
   uint8_t* ws = nullptr;
   size_t ws_bytes = 0;
@@ -1147,12 +1148,13 @@ static int fwd_level(dip_plan* P, int l, cudaStream_t s, int& nl) {
     nl += 2;
   }
   HBM_T(&P->timer, H_BN_ACT_WRITE, 1, (double)nd * ((double)v.h * v.w + (double)(v.h + 2) * (v.w + 2)) * sizeof(float), s,
-        launch_bn_act_write(v.raw_d1, nd, bn_ref(P, v.bn_d1), v.h, v.w, bf ? nullptr : v.P_d1, nd, 1, 1, s, Twin{v.P_d1_16, nd}));
+        launch_bn_act_write(v.raw_d1, nd, bn_ref(P, v.bn_d1), v.h, v.w, bf ? nullptr : v.P_d1, nd, 1, 1, s, Twin{v.P_d1_16, nd},
+                            P->zero_pad));
   DIP_CHECK(v.d2.run_fprop(prec, P->params[v.d2.p_b], s));
   HBM_T(&P->timer, H_BN_ACT_WRITE, last ? 0 : 1,
         (double)nd * ((double)v.h * v.w + (last ? (double)v.h * v.w : (double)(v.h + 2) * (v.w + 2))) * sizeof(float), s,
         launch_bn_act_write(v.raw_d2, nd, bn_ref(P, v.bn_d2), v.h, v.w, (bf && !last && P->lv[l + 1].ns != 4) ? nullptr : v.P_d2, nd, last ? 0 : 1, 1, s,
-                            Twin{last ? nullptr : v.P_d2_16, nd}));   // (the 4-channel skip conv of the next level reads the fp32 tensor)
+                            Twin{last ? nullptr : v.P_d2_16, nd}, P->zero_pad));   // (the 4-channel skip conv of the next level reads the fp32 tensor)
   nl += 4 + (prec == DIP_PRECISION_FP32 ? 2 : 0);
   if (!last) {
     if (deep_on(P) && l + 1 == P->deep_from) {
@@ -1169,7 +1171,7 @@ static int fwd_level(dip_plan* P, int l, cudaStream_t s, int& nl) {
   const double cat_in = ((double)v.cu * v.h * v.w + (double)CS * v.H * v.W) * sizeof(float);
   HBM_T(&P->timer, H_CAT_STATS, v.bilinear, cat_in, s, launch_cat_stats(ca, v.bn_cat.fwd, s));
   HBM_T(&P->timer, H_CAT_WRITE, v.bilinear, cat_in + ((double)v.cu + CS) * (v.H + 2) * (v.W + 2) * sizeof(float), s,
-        launch_cat_write(ca, bn_ref(P, v.bn_cat), v.P_cat, s, Twin{v.P_cat16, v.cat_ld16}));
+        launch_cat_write(ca, bn_ref(P, v.bn_cat), v.P_cat, s, Twin{v.P_cat16, v.cat_ld16}, P->zero_pad));
   DIP_CHECK(v.up.run_fprop(prec, P->params[v.up.p_b], s));
   HBM_T(&P->timer, H_BN_ACT_WRITE, 0, 2.0 * nu * v.H * v.W * sizeof(float), s,
         launch_bn_act_write(v.raw_u, nu, bn_ref(P, v.bn_u), v.H, v.W, bf ? nullptr : v.A_u, nu, 0, 1, s, Twin{v.A_u16, nu}));
@@ -1218,11 +1220,11 @@ static int plan_forward(dip_plan* P, const float* z, const float* noise, float s
   if (P->fnoise.on)
     HBM_T(&P->timer, H_NOISE, 1, ((double)v0.Cin_act * v0.H * v0.W + (double)v0.Cin * (v0.H + 2) * (v0.W + 2)) * sizeof(float), s,
           launch_noise_pad(P->fnoise.z0, P->fnoise.sigma, P->fnoise.seed, P->fnoise.offset, P->fnoise.it_dev, v0.Pin, v0.Cin,
-                           v0.H, v0.W, v0.Cin_act, s, Twin{v0.Pin16, v0.Pin_ld16}));
+                           v0.H, v0.W, v0.Cin_act, s, Twin{v0.Pin16, v0.Pin_ld16}, P->zero_pad));
   else
     HBM_T(&P->timer, H_INPUT_PAD, noise != nullptr,
           ((noise != nullptr ? 2.0 : 1.0) * v0.Cin_act * v0.H * v0.W + (double)v0.Cin * (v0.H + 2) * (v0.W + 2)) * sizeof(float), s,
-          launch_input_pad(z, noise, sigma, v0.Pin, v0.Cin, v0.H, v0.W, s, v0.Cin_act, Twin{v0.Pin16, v0.Pin_ld16}));
+          launch_input_pad(z, noise, sigma, v0.Pin, v0.Cin, v0.H, v0.W, s, v0.Cin_act, Twin{v0.Pin16, v0.Pin_ld16}, P->zero_pad));
   join_side(P, s);
   nl += 3;
   DIP_CHECK(fwd_level(P, 0, s, nl));
@@ -1239,13 +1241,14 @@ static int plan_forward(dip_plan* P, const float* z, const float* noise, float s
 static int bn_bwd(dip_plan* P, const float* raw, int ld_raw, BnLayer& b, int act, GradSrc src, int H, int W, float* draw,
                   float* zs, cudaStream_t s, int& nl, uint16_t* draw16 = nullptr) {
   if (draw16 != nullptr && zs == nullptr) draw = nullptr;   // bf16 mode: only the tensor-core dgrad / wgrad read this gradient
+  if (src.kind == 1) src.zero_pad = P->zero_pad;            // zero padding: the padded gradient's halo is dropped, not folded
   BnRef r = bn_ref(P, b);
   // algorithmic bytes: raw + the gradient source as the kernel's contract names it (plain [H][W][C]; fold: the padded
   // dgrad output (+ the 4-channel skip-branch gradient / the plain addend); upsample adjoint: the 2H x 2W gradient; head:
   // the 4 logit gradients per pixel), + the written input gradient (and its zero-stuffed copy) for the apply pass
   const double px = (double)H * W, C4 = b.C * sizeof(float);
   double gsrc = px * C4;
-  if (src.kind == 1) gsrc = (double)(H + 2) * (W + 2) * C4 + (src.ds != nullptr ? px * 4 * sizeof(float) : 0.0) + (src.add != nullptr ? px * C4 : 0.0);
+  if (src.kind == 1) gsrc = (src.zero_pad ? px : (double)(H + 2) * (W + 2)) * C4 + (src.ds != nullptr ? px * 4 * sizeof(float) : 0.0) + (src.add != nullptr ? px * C4 : 0.0);
   else if (src.kind == 2) gsrc = 4.0 * px * C4;
   else if (src.kind == 3) gsrc = px * 4 * sizeof(float);
   HBM_T(&P->timer, H_BN_BWD_REDUCE, src.kind, px * C4 + gsrc, s, launch_bn_bwd_reduce(raw, ld_raw, r, act, src, H, W, b.bwd, s));
@@ -1326,10 +1329,11 @@ static int bwd_level(dip_plan* P, int l, GradSrc src_v, cudaStream_t s, int& nl)
   }
   // concat BN
   BnRef rc = bn_ref(P, v.bn_cat);
-  const double catb = ((double)v.H * v.W + (double)(v.H + 2) * (v.W + 2)) * CC * sizeof(float);   // stored BN output + padded gradient
-  HBM_T(&P->timer, H_CAT_BWD_REDUCE, 0, catb, s, launch_cat_bwd_reduce(v.P_cat, rc, v.dP_cat, CC, v.H, v.W, v.bn_cat.bwd, s));
+  // stored BN output + padded gradient (zero padding: its interior only)
+  const double catb = ((double)v.H * v.W + (P->zero_pad ? (double)v.H * v.W : (double)(v.H + 2) * (v.W + 2))) * CC * sizeof(float);
+  HBM_T(&P->timer, H_CAT_BWD_REDUCE, 0, catb, s, launch_cat_bwd_reduce(v.P_cat, rc, v.dP_cat, CC, v.H, v.W, v.bn_cat.bwd, s, P->zero_pad));
   HBM_T(&P->timer, H_CAT_BWD_APPLY, 0, catb + (double)v.H * v.W * CC * sizeof(float), s,
-        launch_cat_bwd_apply(v.P_cat, rc, v.dP_cat, CC, v.H, v.W, v.bn_cat.bwd, v.dCat, s));
+        launch_cat_bwd_apply(v.P_cat, rc, v.dP_cat, CC, v.H, v.W, v.bn_cat.bwd, v.dCat, s, P->zero_pad));
   // skip branch (on the skip stream: independent of the deeper levels; the level above joins before it reads dRaw_s / dS)
   cudaStream_t ks = fork_skip(P, s);
   // gradient w.r.t. the low-resolution tensor that was upsampled into this concat (adjoint of x2 upsampling), once
@@ -1531,7 +1535,8 @@ static void deep_bwd_level(dip_plan* P, int l, GradSrc src_v, std::vector<DeepOp
 static int build_deep_ops(dip_plan* P) {
   P->n_deep_fwd = P->n_deep_bwd = 0;
   P->deep_grid = 128 < g_num_sms ? 128 : g_num_sms;
-  if (P->desc.precision != DIP_PRECISION_TF32 || (int)P->lv.size() <= P->deep_from) return 0;
+  // (the op lists write and fold reflection halos only: a zero-padded network keeps the launch-by-launch path)
+  if (P->desc.precision != DIP_PRECISION_TF32 || (int)P->lv.size() <= P->deep_from || P->zero_pad) return 0;
   // the op lists below are written for the 128-wide stride-2 network with the same skip branch (4 or 128 channels) at
   // every scale: they have no pooling pass (downsample_mode 'avg' normalises the pooled raw_d1, which only fwd_level writes)
   for (const Level& v : P->lv)
@@ -1644,26 +1649,42 @@ extern "C" {
 const char* dip_last_error(void) { return g_err.c_str(); }
 int dip_version(void) { return 100; }
 
-size_t dip_plan_workspace_bytes(const dip_net_desc* desc, int H, int W) {
+// options -> plan fields; NULL = defaults (reflection padding)
+static int apply_opts(dip_plan* P, const dip_plan_opts* opts) {
+  const int pad = opts != nullptr ? opts->pad_mode : DIP_PAD_REFLECTION;
+  if (pad != DIP_PAD_REFLECTION && pad != DIP_PAD_ZERO)
+    return fail("dip-b200: pad_mode must be DIP_PAD_REFLECTION (0) or DIP_PAD_ZERO (1), got " + std::to_string(pad));
+  P->zero_pad = pad == DIP_PAD_ZERO;
+  return 0;
+}
+
+size_t dip_plan_workspace_bytes_opts(const dip_net_desc* desc, int H, int W, const dip_plan_opts* opts) {
   dip_plan P;
   P.desc = *desc; P.H = H; P.W = W; P.dry = true;
+  if (apply_opts(&P, opts) != 0) return 0;
   Arena A{nullptr};
   if (build_plan(&P, A) != 0) return 0;
   return A.off + 4096;
 }
+size_t dip_plan_workspace_bytes(const dip_net_desc* desc, int H, int W) { return dip_plan_workspace_bytes_opts(desc, H, W, nullptr); }
 
-int dip_plan_create(const dip_net_desc* desc, int H, int W, void* workspace, size_t workspace_bytes, dip_plan** out) {
+int dip_plan_create_opts(const dip_net_desc* desc, int H, int W, const dip_plan_opts* opts, void* workspace,
+                         size_t workspace_bytes, dip_plan** out) {
   DIP_CHECK(engine_init());
-  const size_t need = dip_plan_workspace_bytes(desc, H, W);
+  const size_t need = dip_plan_workspace_bytes_opts(desc, H, W, opts);
   if (need == 0) return -1;
   if (workspace == nullptr || workspace_bytes < need) return fail("dip_plan_create: workspace too small");
   if (reinterpret_cast<uintptr_t>(workspace) % 256 != 0) return fail("dip_plan_create: workspace must be 256-byte aligned");
   dip_plan* P = new dip_plan();
   P->desc = *desc; P->H = H; P->W = W; P->ws = (uint8_t*)workspace; P->ws_bytes = workspace_bytes;
+  apply_opts(P, opts);
   Arena A{(uint8_t*)workspace};
   if (build_plan(P, A) != 0) { delete P; return -1; }
   *out = P;
   return 0;
+}
+int dip_plan_create(const dip_net_desc* desc, int H, int W, void* workspace, size_t workspace_bytes, dip_plan** out) {
+  return dip_plan_create_opts(desc, H, W, nullptr, workspace, workspace_bytes, out);
 }
 void dip_plan_destroy(dip_plan* plan) {
   if (plan == nullptr) return;
@@ -1924,7 +1945,7 @@ int dip_run_iterations(dip_plan* P, dip_adam* adam, const void* z0, const void* 
 int dip_input_grad(dip_plan* P, void* dz, dip_stream_t stream) {
   if (!P->desc.input_grad) return fail("dip_input_grad: the plan was created without input_grad");
   Level& v = P->lv[0];
-  launch_input_grad(v.dPin, v.ns > 0 ? v.dS : nullptr, v.Cin, v.Cin_act, v.H, v.W, (float*)dz, (cudaStream_t)stream);
+  launch_input_grad(v.dPin, v.ns > 0 ? v.dS : nullptr, v.Cin, v.Cin_act, v.H, v.W, (float*)dz, (cudaStream_t)stream, P->zero_pad);
   DIP_CUDA(cudaGetLastError());
   return 0;
 }

@@ -103,8 +103,10 @@ struct HeadRef {
 
 // z (NCHW, C x H x W) [+ sigma * noise (NCHW)] -> reflection-padded NHWC [(H+2)][(W+2)][C]
 // C = stored depth of dst; c_src (0: C) = depth of z / noise, the remaining channels are written as zeros
+// zero_pad = 1: the halo ring is written as zeros (Conv2d(padding=1) instead of ReflectionPad2d(1)); the same switch on
+// every launcher below that writes or folds a halo
 void launch_input_pad(const float* z, const float* noise, float sigma, float* dst, int C, int H, int W,
-                      cudaStream_t s, int c_src = 0, Twin t16 = kNoTwin);
+                      cudaStream_t s, int c_src = 0, Twin t16 = kNoTwin, int zero_pad = 0);
 
 // generic per-channel sum / sum^2 of a plain NHWC tensor (SIMT-conv path and skinny convs)
 void launch_channel_stats(const float* x, int ld, int C, int npix, double* fwd, cudaStream_t s);
@@ -112,7 +114,7 @@ void launch_channel_stats(const float* x, int ld, int C, int npix, double* fwd, 
 // y = lrelu(bn(x)) written plain [H][W][ld_out] or reflection padded [(H+2)][(W+2)][ld_out]
 // dst may be null when a bf16 twin is given (the tensor is then only read by tensor-core kernels)
 void launch_bn_act_write(const float* raw, int ld_in, BnRef bn, int H, int W, float* dst, int ld_out, int pad,
-                         int act, cudaStream_t s, Twin t16 = kNoTwin);
+                         int act, cudaStream_t s, Twin t16 = kNoTwin, int zero_pad = 0);
 // y = lrelu(bn(x)) consumed on the fly by the RGB head (C must be 128); y itself is not materialised
 void launch_bn_act_head(const float* raw, BnRef bn, int H, int W, HeadRef head, cudaStream_t s);
 
@@ -126,7 +128,7 @@ struct CatArgs {
 };
 void launch_cat_stats(CatArgs a, double* fwd_cat, cudaStream_t s);
 // dst = bn_cat(cat) with reflection pad: [(H+2)][(W+2)][Cu+Cs]
-void launch_cat_write(CatArgs a, BnRef bn_cat, float* dst, cudaStream_t s, Twin t16 = kNoTwin);
+void launch_cat_write(CatArgs a, BnRef bn_cat, float* dst, cudaStream_t s, Twin t16 = kNoTwin, int zero_pad = 0);
 
 // Gradient sources for the BN backward kernels
 struct GradSrc {
@@ -145,6 +147,9 @@ struct GradSrc {
   const float* dl4;    // [npix][4] logit gradients dout * o * (1 - o) (launch_head_dlogit)
   const float* wh;     // [K][C]
   int nh;
+  // kind 1: adjoint of zero padding (the halo of g is dropped) instead of the reflection fold.  (Placed in the alignment gap
+  // after nh: the struct's size and the offsets of the other fields stay those of the reflection-only layout.)
+  int zero_pad;
   double* dwh;         // [K][C] fp64 accumulators (reduce pass)
   double* dbh;         // [K]
 };
@@ -155,7 +160,8 @@ void launch_head_dlogit(const float* dout, const float* outv, int K, int npix, f
 // dL/dz of the network input (OPT_OVER='input', utils/common_utils.py:47-49), torch layout [C][H][W]:
 //   dz[c][i][j] = fold(gp)[i][j][c] + ds[i][j][c]; gp = padded dgrad output of the level-0 stride-2 conv
 //   [(H+2)][(W+2)][ld], ds = input gradient of the level-0 skip conv [H][W][ld] (nullable)
-void launch_input_grad(const float* gp, const float* ds, int ld, int C, int H, int W, float* dz, cudaStream_t s);
+void launch_input_grad(const float* gp, const float* ds, int ld, int C, int H, int W, float* dz, cudaStream_t s,
+                       int zero_pad = 0);
 
 // BN(+LeakyReLU) backward. reduce: bwd[0..C) += sum dz, bwd[C..2C) += sum dz*xhat.
 // apply: dx = gamma*rstd*(dz - mean(dz) - xhat*mean(dz*xhat)); writes draw plain [H][W][C];
@@ -174,9 +180,9 @@ void launch_avgpool2_bwd(const float* dy, int h, int w, int C, float* dx, cudaSt
 // Concat-BN backward (no activation). pcat = the stored BN output (padded [(H+2)][(W+2)][ld], ld = bn_cat.C), from which
 // xhat is recovered; gradient = fold of the padded dgrad output gp [(H+2)][(W+2)][ld]; dcat plain [H][W][C].
 void launch_cat_bwd_reduce(const float* pcat, BnRef bn_cat, const float* gp, int ld, int H, int W, double* bwd,
-                           cudaStream_t s);
+                           cudaStream_t s, int zero_pad = 0);
 void launch_cat_bwd_apply(const float* pcat, BnRef bn_cat, const float* gp, int ld, int H, int W, const double* bwd,
-                          float* dcat, cudaStream_t s);
+                          float* dcat, cudaStream_t s, int zero_pad = 0);
 // adjoint of the x2 upsampling, once per level: dst[h][w][C] <- D[2h][2w][ld] channels [coff, coff+C)
 void launch_upadj(const float* D, int ld, int coff, int h, int w, int C, int bilinear, float* dst, cudaStream_t s);
 
@@ -205,7 +211,7 @@ void launch_noise(const float* z0, float* z, float sigma, uint64_t seed, uint64_
 // runner input in one pass: dst (reflection-padded NHWC [(H+2)][(W+2)][C]) = pad(z0 + sigma * N(0,1)), the same Philox stream
 // as launch_noise (W % 4 == 0); channels >= c_src of the stored depth C are written as zeros
 void launch_noise_pad(const float* z0, float sigma, uint64_t seed, uint64_t offset, const int* it_dev, float* dst, int C, int H,
-                      int W, int c_src, cudaStream_t s, Twin t16 = kNoTwin);
+                      int W, int c_src, cudaStream_t s, Twin t16 = kNoTwin, int zero_pad = 0);
 // it_dev[0] += 1, it_dev[1] += 1 (step / iteration counters of the graph-captured runner)
 void launch_advance(int* it_dev, cudaStream_t s);
 

@@ -4,6 +4,7 @@
 // (models/skip.py:41-100 built from models/common.py:76-124):
 //   input_pad        : net_input perturbation + nn.ReflectionPad2d(1)            (denoising.ipynb c10:12-13, common.py:117)
 //   bn_act_write     : nn.BatchNorm2d (training mode) + nn.LeakyReLU(0.2) + nn.ReflectionPad2d(1)   (common.py:96,82,117)
+//                      (pad != 'reflection': the zero halo of Conv2d(padding=1) instead, in every halo writer / fold below)
 //   bn_act_head      : last BN + LeakyReLU + 1x1 conv 128->3 + nn.Sigmoid in one pass (skip.py:90-98)
 //   cat_stats/write  : nn.Upsample(x2) + Concat + nn.BatchNorm2d(132) + pad     (skip.py:81,50-55; common.py:19-39)
 //   bn_bwd_*/cat_bwd_*: autograd adjoints of the above, with the producer of the incoming gradient fused in
@@ -218,21 +219,24 @@ static void fit_grid(VecGeom& g, Kern kernel, size_t smem) {
 }
 
 // ------------------------------------------------------------------------------------------------ input_pad
+// ZP (zero padding, Conv2d(padding=1)): the halo ring is written as zeros instead of the mirrored pixels.  Every kernel
+// that writes or folds a halo takes ZP as a template parameter, so the reflection instantiation is the unchanged code.
+template <bool ZP>
 __global__ void k_input_pad(const float* __restrict__ z, const float* __restrict__ noise, float sigma,
                             float* __restrict__ dst, int C, int H, int W, int Cs, Twin t16) {
   pdl_enter();
   __shared__ float tile[32][33];
   const int Wp = W + 2;
   const int yy = blockIdx.y;
-  const int sy = reflect_idx(yy - 1, H);
+  const int sy = ZP ? yy - 1 : reflect_idx(yy - 1, H);
   const int tx = threadIdx.x, ty = threadIdx.y;
   for (int c0 = 0; c0 < C; c0 += 32) {
     const int xx = blockIdx.x * 32 + tx;
     for (int k = 0; k < 4; ++k) {
       const int c = c0 + ty + 8 * k;
       float val = 0.f;
-      if (xx < Wp && c < Cs) {
-        const int sx = reflect_idx(xx - 1, W);
+      if (xx < Wp && c < Cs && (!ZP || (sy >= 0 && sy < H && xx >= 1 && xx <= W))) {
+        const int sx = ZP ? xx - 1 : reflect_idx(xx - 1, W);
         const size_t off = (static_cast<size_t>(c) * H + sy) * W + sx;
         val = z[off];
         if (noise != nullptr) val = fmaf(noise[off], sigma, val);
@@ -252,9 +256,10 @@ __global__ void k_input_pad(const float* __restrict__ z, const float* __restrict
   }
 }
 void launch_input_pad(const float* z, const float* noise, float sigma, float* dst, int C, int H, int W,
-                      cudaStream_t s, int c_src, Twin t16) {
+                      cudaStream_t s, int c_src, Twin t16, int zero_pad) {
   dim3 grid((W + 2 + 31) / 32, H + 2), block(32, 8);
-  launch_k(k_input_pad, dim3(grid), dim3(block), 0, s, 1, z, noise, sigma, dst, C, H, W, c_src > 0 ? c_src : C, t16);
+  launch_k(zero_pad ? k_input_pad<true> : k_input_pad<false>, dim3(grid), dim3(block), 0, s, 1, z, noise, sigma, dst, C, H, W,
+           c_src > 0 ? c_src : C, t16);
 }
 
 // ------------------------------------------------------------------------------------------------ cast (single ops)
@@ -317,6 +322,8 @@ void launch_channel_stats(const float* x, int ld, int C, int npix, double* fwd, 
 }
 
 // ------------------------------------------------------------------------------------------------ bn_act_write
+// ZP: with pad, the halo cells are written as 0 (their load reads the nearest interior pixel, whose value is discarded)
+template <bool ZP = false>
 __device__ __forceinline__ void d_bn_act_write(const float* __restrict__ raw, int ld_in, BnRef bn, int H, int W,
                                                       float* __restrict__ dst, int ld_out, int pad, int act, int VL,
                                                       int PPB, Twin t16 = kNoTwin) {
@@ -326,28 +333,34 @@ __device__ __forceinline__ void d_bn_act_write(const float* __restrict__ raw, in
   item_loop<4>(blockIdx.x * PPB + slot, gridDim.x * PPB, Ho * Wo,
                [&](int p) {
                  const int yo = p / Wo, xo = p - yo * Wo;
-                 const int yi = pad ? reflect_idx(yo - 1, H) : yo;
-                 const int xi = pad ? reflect_idx(xo - 1, W) : xo;
+                 const int yi = pad ? (ZP ? min(max(yo - 1, 0), H - 1) : reflect_idx(yo - 1, H)) : yo;
+                 const int xi = pad ? (ZP ? min(max(xo - 1, 0), W - 1) : reflect_idx(xo - 1, W)) : xo;
                  return ld4(raw + (static_cast<size_t>(yi) * W + xi) * ld_in + 4 * v);
                },
                [&](int p, float4 x) {
                  float4 y = bn_apply(cf, x);
                  if (act) y = lrelu4(y);
+                 if (ZP && pad) {
+                   const int yo = p / Wo, xo = p - yo * Wo;
+                   if (yo == 0 || yo == Ho - 1 || xo == 0 || xo == Wo - 1) y = f4zero();
+                 }
                  if (dst != nullptr) st4(dst + static_cast<size_t>(p) * ld_out + 4 * v, y);
                  if (t16.p != nullptr) st4_bf16(t16.p + static_cast<size_t>(p) * t16.ld + 4 * v, y);
                });
 }
+template <bool ZP>
 __global__ void __launch_bounds__(256) k_bn_act_write(const float* __restrict__ raw, int ld_in, BnRef bn, int H, int W,
                                                       float* __restrict__ dst, int ld_out, int pad, int act, int VL,
                                                       int PPB, Twin t16) {
   pdl_enter();
-  d_bn_act_write(raw, ld_in, bn, H, W, dst, ld_out, pad, act, VL, PPB, t16);
+  d_bn_act_write<ZP>(raw, ld_in, bn, H, W, dst, ld_out, pad, act, VL, PPB, t16);
 }
 void launch_bn_act_write(const float* raw, int ld_in, BnRef bn, int H, int W, float* dst, int ld_out, int pad,
-                         int act, cudaStream_t s, Twin t16) {
+                         int act, cudaStream_t s, Twin t16, int zero_pad) {
   VecGeom g = vec_geom(bn.C, static_cast<long long>(H + 2 * pad) * (W + 2 * pad));
-  fit_grid(g, k_bn_act_write, 0);
-  launch_k(k_bn_act_write, dim3(g.blocks), dim3(g.threads), 0, s, 1, raw, ld_in, bn, H, W, dst, ld_out, pad, act, g.VL, g.PPB, t16);
+  auto kernel = zero_pad && pad ? k_bn_act_write<true> : k_bn_act_write<false>;
+  fit_grid(g, kernel, 0);
+  launch_k(kernel, dim3(g.blocks), dim3(g.threads), 0, s, 1, raw, ld_in, bn, H, W, dst, ld_out, pad, act, g.VL, g.PPB, t16);
 }
 
 // BN + LeakyReLU + RGB head + sigmoid: one warp per pixel (C = 128 -> 32 lanes x float4), nothing but out is written.
@@ -471,24 +484,29 @@ void launch_cat_stats(CatArgs a, double* fwd_cat, cudaStream_t s) {
 }
 
 // store the value of interior pixel (i, j) at its padded position and at every halo position that mirrors it
+// (ZP: the border pixels of the image write the zeros of the halo cells next to them instead; the corner pixels also
+// write the halo corner)
+template <bool ZP = false>
 __device__ __forceinline__ void store_with_halo(float* __restrict__ dst, int ld, int H, int W, int i, int j, int v, float4 val,
                                                 Twin t16 = kNoTwin) {
   int rows[3], cols[3];
   int nr = 0, nc = 0;
   rows[nr++] = i + 1;
-  if (i == 1) rows[nr++] = 0;
-  if (i == H - 2) rows[nr++] = H + 1;
+  if (i == (ZP ? 0 : 1)) rows[nr++] = 0;
+  if (i == (ZP ? H - 1 : H - 2)) rows[nr++] = H + 1;
   cols[nc++] = j + 1;
-  if (j == 1) cols[nc++] = 0;
-  if (j == W - 2) cols[nc++] = W + 1;
+  if (j == (ZP ? 0 : 1)) cols[nc++] = 0;
+  if (j == (ZP ? W - 1 : W - 2)) cols[nc++] = W + 1;
   const int Wp = W + 2;
   for (int r = 0; r < nr; ++r)
     for (int c = 0; c < nc; ++c) {
-      st4(dst + (static_cast<size_t>(rows[r]) * Wp + cols[c]) * ld + 4 * v, val);
-      if (t16.p != nullptr) st4_bf16(t16.p + (static_cast<size_t>(rows[r]) * Wp + cols[c]) * t16.ld + 4 * v, val);
+      const float4 o = ZP && (r > 0 || c > 0) ? f4zero() : val;
+      st4(dst + (static_cast<size_t>(rows[r]) * Wp + cols[c]) * ld + 4 * v, o);
+      if (t16.p != nullptr) st4_bf16(t16.p + (static_cast<size_t>(rows[r]) * Wp + cols[c]) * t16.ld + 4 * v, o);
     }
 }
 
+template <bool ZP = false>
 __device__ __forceinline__ void d_cat_write(CatArgs a, BnRef bn_cat, float* __restrict__ dst, int VL, int PPB, Twin t16 = kNoTwin) {
   const int v = threadIdx.x % VL, slot = threadIdx.x / VL;
   const CatLane l = cat_lane(a, v);
@@ -501,21 +519,25 @@ __device__ __forceinline__ void d_cat_write(CatArgs a, BnRef bn_cat, float* __re
     cat_quad(a, l, si, sj, v, q);
 #pragma unroll
     for (int e = 0; e < 4; ++e)
-      store_with_halo(dst, ld, a.H, a.W, 2 * si + (e >> 1), 2 * sj + (e & 1), v, bn_apply(cf, q[e]), t16);
+      store_with_halo<ZP>(dst, ld, a.H, a.W, 2 * si + (e >> 1), 2 * sj + (e & 1), v, bn_apply(cf, q[e]), t16);
   }
 }
+template <bool ZP>
 __global__ void __launch_bounds__(256, DIP_CAT_MINBLOCKS) k_cat_write(CatArgs a, BnRef bn_cat, float* __restrict__ dst, int VL, int PPB, Twin t16) {
   pdl_enter();
-  d_cat_write(a, bn_cat, dst, VL, PPB, t16);
+  d_cat_write<ZP>(a, bn_cat, dst, VL, PPB, t16);
 }
-void launch_cat_write(CatArgs a, BnRef bn_cat, float* dst, cudaStream_t s, Twin t16) {
+void launch_cat_write(CatArgs a, BnRef bn_cat, float* dst, cudaStream_t s, Twin t16, int zero_pad) {
   VecGeom g = vec_geom(a.Cu + a.Cs, static_cast<long long>(a.H / 2) * (a.W / 2));
-  fit_grid(g, k_cat_write, 0);
-  launch_k(k_cat_write, dim3(g.blocks), dim3(g.threads), 0, s, 1, a, bn_cat, dst, g.VL, g.PPB, t16);
+  auto kernel = zero_pad ? k_cat_write<true> : k_cat_write<false>;
+  fit_grid(g, kernel, 0);
+  launch_k(kernel, dim3(g.blocks), dim3(g.threads), 0, s, 1, a, bn_cat, dst, g.VL, g.PPB, t16);
 }
 
 // ------------------------------------------------------------------------------------------------ gradient sources
 // fold: adjoint of ReflectionPad2d(1). Interior (i,j) <- padded (i+1,j+1) plus mirrored halo rows/cols.
+// ZP: adjoint of zero padding: the interior position only (the halo's gradient is dropped)
+template <bool ZP = false>
 __device__ __forceinline__ float4 fold_read(const float* __restrict__ gp, int ld, int coff, int H, int W, int i, int j,
                                             int v) {
   const int Wp = W + 2;
@@ -523,7 +545,7 @@ __device__ __forceinline__ float4 fold_read(const float* __restrict__ gp, int ld
   // the interior load is unconditional (issued at once, so several items' loads are in flight together); only the
   // one-pixel ring next to the border has mirrored halo positions to add
   float4 r = ld4(base + (static_cast<size_t>(i + 1) * Wp + (j + 1)) * ld);
-  if (i == 1 || i == H - 2 || j == 1 || j == W - 2) {
+  if (!ZP && (i == 1 || i == H - 2 || j == 1 || j == W - 2)) {
     int rows[3], cols[3];
     int nr = 0, nc = 0;
     rows[nr++] = i + 1;
@@ -638,10 +660,12 @@ __device__ __forceinline__ void row_loop(int H, int W, int PPB, int slot, Load l
       if (j0 + u * PPB < W) use(i, j0 + u * PPB, u);
   }
 }
-// mirrored halo positions of interior pixel (i, j) added to its interior value r (fold = adjoint of ReflectionPad2d(1))
+// mirrored halo positions of interior pixel (i, j) added to its interior value r (fold = adjoint of ReflectionPad2d(1));
+// ZP (adjoint of zero padding): nothing is added
+template <bool ZP = false>
 __device__ __forceinline__ float4 fold_border(const float* __restrict__ gp, int ld, int coff, int H, int W, int i, int j, int v,
                                               float4 r) {
-  if (i == 1 || i == H - 2 || j == 1 || j == W - 2) {
+  if (!ZP && (i == 1 || i == H - 2 || j == 1 || j == W - 2)) {
     const int Wp = W + 2;
     const float* base = gp + coff + 4 * v;
     const int r2 = i == 1 ? 0 : (i == H - 2 ? H + 1 : -1), c2 = j == 1 ? 0 : (j == W - 2 ? W + 1 : -1);
@@ -672,9 +696,10 @@ __device__ __forceinline__ void fold_item_load(const GradSrc& s, const float* __
   if (s.ds != nullptr) it.d = ld4(s.ds + p * 4);
   else if (s.add != nullptr) it.d = ld4(s.add + p * s.ld_add + 4 * v);
 }
+template <bool ZP = false>
 __device__ __forceinline__ float4 fold_item_grad(const GradSrc& s, const SrcRegs& sr, int H, int W, int i, int j, int v,
                                                  const FoldItem& it) {
-  float4 r = fold_border(s.g, s.ld, s.coff, H, W, i, j, v, it.g);
+  float4 r = fold_border<ZP>(s.g, s.ld, s.coff, H, W, i, j, v, it.g);
   if (s.ds != nullptr) {   // + the input gradient of the next level's 1x1 skip conv, computed on the fly
     r = f4fma(it.d.x, sr.w[0], r);
     r = f4fma(it.d.y, sr.w[1], r);
@@ -710,7 +735,9 @@ void launch_head_dlogit(const float* dout, const float* outv, int K, int npix, f
 
 // ------------------------------------------------------------------------------------------------ input gradient
 // NHWC -> NCHW transpose through a 32 x 32 shared tile (rows of 32 pixels of one image row x 32 channels), with the
-// reflection-pad adjoint of the padded gradient and the skip-conv addend applied while reading.
+// reflection-pad adjoint of the padded gradient and the skip-conv addend applied while reading (ZP: the zero-pad
+// adjoint, the interior of the padded gradient only).
+template <bool ZP>
 __global__ void k_input_grad(const float* __restrict__ gp, const float* __restrict__ ds, int ld, int C, int H, int W,
                              float* __restrict__ dz) {
   pdl_enter();
@@ -726,11 +753,11 @@ __global__ void k_input_grad(const float* __restrict__ gp, const float* __restri
         int rows[3], cols[3];
         int nr = 0, nc = 0;
         rows[nr++] = i + 1;
-        if (i == 1) rows[nr++] = 0;
-        if (i == H - 2) rows[nr++] = H + 1;
+        if (!ZP && i == 1) rows[nr++] = 0;
+        if (!ZP && i == H - 2) rows[nr++] = H + 1;
         cols[nc++] = j + 1;
-        if (j == 1) cols[nc++] = 0;
-        if (j == W - 2) cols[nc++] = W + 1;
+        if (!ZP && j == 1) cols[nc++] = 0;
+        if (!ZP && j == W - 2) cols[nc++] = W + 1;
         for (int a = 0; a < nr; ++a)
           for (int b = 0; b < nc; ++b) val += gp[(static_cast<size_t>(rows[a]) * Wp + cols[b]) * ld + c];
         if (ds != nullptr) val += ds[(static_cast<size_t>(i) * W + j) * ld + c];
@@ -745,11 +772,12 @@ __global__ void k_input_grad(const float* __restrict__ gp, const float* __restri
     __syncthreads();
   }
 }
-void launch_input_grad(const float* gp, const float* ds, int ld, int C, int H, int W, float* dz, cudaStream_t s) {
+void launch_input_grad(const float* gp, const float* ds, int ld, int C, int H, int W, float* dz, cudaStream_t s, int zero_pad) {
   dim3 grid((W + 31) / 32, H), block(32, 8);
-  launch_k(k_input_grad, dim3(grid), dim3(block), 0, s, 1, gp, ds, ld, C, H, W, dz);
+  launch_k(zero_pad ? k_input_grad<true> : k_input_grad<false>, dim3(grid), dim3(block), 0, s, 1, gp, ds, ld, C, H, W, dz);
 }
-template <int KIND>
+// ZP applies to KIND 1 only: the padded gradient's halo is dropped instead of folded (zero-padding adjoint)
+template <int KIND, bool ZP = false>
 __device__ __forceinline__ void d_bn_bwd_reduce(const float* __restrict__ raw, int ld_raw, BnRef bn, int act, GradSrc src,
                                                        int H, int W, double* __restrict__ bwd, int VL, int PPB) {
   const int v = threadIdx.x % VL, slot = threadIdx.x / VL;
@@ -761,7 +789,7 @@ __device__ __forceinline__ void d_bn_bwd_reduce(const float* __restrict__ raw, i
     row_loop<DIP_U_BWD1>(H, W, PPB, slot,
                          [&](int i, int j, int u) { fold_item_load(src, raw, ld_raw, W, i, j, v, it[u]); },
                          [&](int i, int j, int u) {
-                           float4 dz = fold_item_grad(src, sr, H, W, i, j, v, it[u]);
+                           float4 dz = fold_item_grad<ZP>(src, sr, H, W, i, j, v, it[u]);
                            if (act) dz = lrelu_bwd4(bn_apply(cf, it[u].x), dz);
                            acc[0] = f4add(acc[0], dz);
                            acc[1] = f4mla(dz, bn_xhat(cf, it[u].x), acc[1]);
@@ -786,29 +814,26 @@ __device__ __forceinline__ void d_bn_bwd_reduce(const float* __restrict__ raw, i
   const int wid[2] = {bn.C, bn.C};
   block_reduce_atomic<2>(acc, VL, PPB, dst, wid);
 }
-template <int KIND>
+template <int KIND, bool ZP = false>
 __global__ void __launch_bounds__(256, (KIND == 0 || KIND == 2) ? 3 : 2) k_bn_bwd_reduce(const float* __restrict__ raw, int ld_raw, BnRef bn, int act, GradSrc src,
                                                        int H, int W, double* __restrict__ bwd, int VL, int PPB) {
   pdl_enter();
-  d_bn_bwd_reduce<KIND>(raw, ld_raw, bn, act, src, H, W, bwd, VL, PPB);
+  d_bn_bwd_reduce<KIND, ZP>(raw, ld_raw, bn, act, src, H, W, bwd, VL, PPB);
 }
 void launch_bn_bwd_reduce(const float* raw, int ld_raw, BnRef bn, int act, GradSrc src, int H, int W, double* bwd,
                           cudaStream_t s) {
   VecGeom g = vec_geom(bn.C, static_cast<long long>(H) * W);
   const size_t sm = red_bytes(g, 2);
-  if (src.kind == 0) fit_grid(g, k_bn_bwd_reduce<0>, sm);
-  else if (src.kind == 1) fit_grid(g, k_bn_bwd_reduce<1>, sm);
-  else if (src.kind == 2) fit_grid(g, k_bn_bwd_reduce<2>, sm);
-  else fit_grid(g, k_bn_bwd_reduce<3>, sm);
-  if (src.kind == 0) launch_red(k_bn_bwd_reduce<0>, g.blocks, g.threads, sm, s, raw, ld_raw, bn, act, src, H, W, bwd, g.VL, g.PPB);
-  else if (src.kind == 1) launch_red(k_bn_bwd_reduce<1>, g.blocks, g.threads, sm, s, raw, ld_raw, bn, act, src, H, W, bwd, g.VL, g.PPB);
-  else if (src.kind == 2) launch_red(k_bn_bwd_reduce<2>, g.blocks, g.threads, sm, s, raw, ld_raw, bn, act, src, H, W, bwd, g.VL, g.PPB);
-  else launch_red(k_bn_bwd_reduce<3>, g.blocks, g.threads, sm, s, raw, ld_raw, bn, act, src, H, W, bwd, g.VL, g.PPB);
+  auto kernel = src.kind == 0 ? k_bn_bwd_reduce<0>
+              : src.kind == 1 ? (src.zero_pad ? k_bn_bwd_reduce<1, true> : k_bn_bwd_reduce<1>)
+              : src.kind == 2 ? k_bn_bwd_reduce<2> : k_bn_bwd_reduce<3>;
+  fit_grid(g, kernel, sm);
+  launch_red(kernel, g.blocks, g.threads, sm, s, raw, ld_raw, bn, act, src, H, W, bwd, g.VL, g.PPB);
 }
 
 // apply pass; for the head source (KIND 3) it also accumulates the head's own gradients:
 //   dW_head[k][c] += dl[k] * act(bn(raw))[c],  db_head[k] += dl[k]
-template <int KIND>
+template <int KIND, bool ZP = false>
 __device__ __forceinline__ void d_bn_bwd_apply(const float* __restrict__ raw, int ld_raw, BnRef bn, int act, GradSrc src,
                                                       int H, int W, const double* __restrict__ bwd, float* __restrict__ draw,
                                                       float* __restrict__ zs, double* __restrict__ dbias, int VL, int PPB,
@@ -828,7 +853,7 @@ __device__ __forceinline__ void d_bn_bwd_apply(const float* __restrict__ raw, in
     row_loop<DIP_U_BWD1>(H, W, PPB, slot,
                          [&](int i, int j, int u) { fold_item_load(src, raw, ld_raw, W, i, j, v, it[u]); },
                          [&](int i, int j, int u) {
-                           float4 dz = fold_item_grad(src, sr, H, W, i, j, v, it[u]);
+                           float4 dz = fold_item_grad<ZP>(src, sr, H, W, i, j, v, it[u]);
                            if (act) dz = lrelu_bwd4(bn_apply(cf, it[u].x), dz);
                            const float4 xh = bn_xhat(cf, it[u].x);
                            float4 dx;
@@ -890,24 +915,22 @@ __device__ __forceinline__ void d_bn_bwd_apply(const float* __restrict__ raw, in
     block_reduce_atomic<K>(acc, VL, PPB, dst, wid);
   }
 }
-template <int KIND>
+template <int KIND, bool ZP = false>
 __global__ void __launch_bounds__(256, KIND == 2 ? 3 : 2) k_bn_bwd_apply(const float* __restrict__ raw, int ld_raw, BnRef bn, int act, GradSrc src,
                                                       int H, int W, const double* __restrict__ bwd, float* __restrict__ draw,
                                                       float* __restrict__ zs, double* __restrict__ dbias, int VL, int PPB, Twin t16) {
   pdl_enter();
-  d_bn_bwd_apply<KIND>(raw, ld_raw, bn, act, src, H, W, bwd, draw, zs, dbias, VL, PPB, t16);
+  d_bn_bwd_apply<KIND, ZP>(raw, ld_raw, bn, act, src, H, W, bwd, draw, zs, dbias, VL, PPB, t16);
 }
 void launch_bn_bwd_apply(const float* raw, int ld_raw, BnRef bn, int act, GradSrc src, int H, int W,
                          const double* bwd, float* draw, float* zs, double* dbias, cudaStream_t s, Twin t16) {
   VecGeom g = vec_geom(bn.C, static_cast<long long>(H) * W);
-  if (src.kind == 0) fit_grid(g, k_bn_bwd_apply<0>, red_bytes(g, 1));
-  else if (src.kind == 1) fit_grid(g, k_bn_bwd_apply<1>, red_bytes(g, 1));
-  else if (src.kind == 2) fit_grid(g, k_bn_bwd_apply<2>, red_bytes(g, 1));
-  else fit_grid(g, k_bn_bwd_apply<3>, red_bytes(g, 6));
-  if (src.kind == 0) launch_red(k_bn_bwd_apply<0>, g.blocks, g.threads, red_bytes(g, 1), s, raw, ld_raw, bn, act, src, H, W, bwd, draw, zs, dbias, g.VL, g.PPB, t16);
-  else if (src.kind == 1) launch_red(k_bn_bwd_apply<1>, g.blocks, g.threads, red_bytes(g, 1), s, raw, ld_raw, bn, act, src, H, W, bwd, draw, zs, dbias, g.VL, g.PPB, t16);
-  else if (src.kind == 2) launch_red(k_bn_bwd_apply<2>, g.blocks, g.threads, red_bytes(g, 1), s, raw, ld_raw, bn, act, src, H, W, bwd, draw, zs, dbias, g.VL, g.PPB, t16);
-  else launch_red(k_bn_bwd_apply<3>, g.blocks, g.threads, red_bytes(g, 6), s, raw, ld_raw, bn, act, src, H, W, bwd, draw, zs, dbias, g.VL, g.PPB, t16);
+  const size_t sm = red_bytes(g, src.kind == 3 ? 6 : 1);
+  auto kernel = src.kind == 0 ? k_bn_bwd_apply<0>
+              : src.kind == 1 ? (src.zero_pad ? k_bn_bwd_apply<1, true> : k_bn_bwd_apply<1>)
+              : src.kind == 2 ? k_bn_bwd_apply<2> : k_bn_bwd_apply<3>;
+  fit_grid(g, kernel, sm);
+  launch_red(kernel, g.blocks, g.threads, sm, s, raw, ld_raw, bn, act, src, H, W, bwd, draw, zs, dbias, g.VL, g.PPB, t16);
 }
 
 // ------------------------------------------------------------------------------------------------ concat-BN backward
@@ -940,6 +963,7 @@ __device__ __forceinline__ float4 cat_xhat(const CatBwdCoef& c, float4 y) {
   return make_float4((y.x - c.beta.x) * c.inv_gamma.x, (y.y - c.beta.y) * c.inv_gamma.y, (y.z - c.beta.z) * c.inv_gamma.z,
                      (y.w - c.beta.w) * c.inv_gamma.w);
 }
+template <bool ZP = false>
 __device__ __forceinline__ void d_cat_bwd_reduce(const float* __restrict__ pcat, BnRef bn_cat, const float* __restrict__ gp,
                                                         int ld, int H, int W, double* __restrict__ bwd, int VL, int PPB) {
   const int v = threadIdx.x % VL, slot = threadIdx.x / VL;
@@ -952,7 +976,7 @@ __device__ __forceinline__ void d_cat_bwd_reduce(const float* __restrict__ pcat,
                  RedItem it;
                  const int i = p / W, j = p - i * W;
                  it.x = ld4(pcat + (static_cast<size_t>(i + 1) * Wp + (j + 1)) * ld + 4 * v);
-                 it.g = fold_read(gp, ld, 0, H, W, i, j, v);
+                 it.g = fold_read<ZP>(gp, ld, 0, H, W, i, j, v);
                  return it;
                },
                [&](int, const RedItem& it) {
@@ -963,17 +987,20 @@ __device__ __forceinline__ void d_cat_bwd_reduce(const float* __restrict__ pcat,
   const int wid[2] = {bn_cat.C, bn_cat.C};
   block_reduce_atomic<2>(acc, VL, PPB, dst, wid);
 }
+template <bool ZP>
 __global__ void __launch_bounds__(256) k_cat_bwd_reduce(const float* __restrict__ pcat, BnRef bn_cat, const float* __restrict__ gp,
                                                         int ld, int H, int W, double* __restrict__ bwd, int VL, int PPB) {
   pdl_enter();
-  d_cat_bwd_reduce(pcat, bn_cat, gp, ld, H, W, bwd, VL, PPB);
+  d_cat_bwd_reduce<ZP>(pcat, bn_cat, gp, ld, H, W, bwd, VL, PPB);
 }
 void launch_cat_bwd_reduce(const float* pcat, BnRef bn_cat, const float* gp, int ld, int H, int W, double* bwd,
-                           cudaStream_t s) {
+                           cudaStream_t s, int zero_pad) {
   VecGeom g = vec_geom(bn_cat.C, static_cast<long long>(H) * W);
-  fit_grid(g, k_cat_bwd_reduce, red_bytes(g, 2));
-  launch_red(k_cat_bwd_reduce, g.blocks, g.threads, red_bytes(g, 2), s, pcat, bn_cat, gp, ld, H, W, bwd, g.VL, g.PPB);
+  auto kernel = zero_pad ? k_cat_bwd_reduce<true> : k_cat_bwd_reduce<false>;
+  fit_grid(g, kernel, red_bytes(g, 2));
+  launch_red(kernel, g.blocks, g.threads, red_bytes(g, 2), s, pcat, bn_cat, gp, ld, H, W, bwd, g.VL, g.PPB);
 }
+template <bool ZP = false>
 __device__ __forceinline__ void d_cat_bwd_apply(const float* __restrict__ pcat, BnRef bn_cat, const float* __restrict__ gp,
                                                        int ld, int H, int W, const double* __restrict__ bwd,
                                                        float* __restrict__ dcat, int VL, int PPB) {
@@ -988,7 +1015,7 @@ __device__ __forceinline__ void d_cat_bwd_apply(const float* __restrict__ pcat, 
                  RedItem it;
                  const int i = p / W, j = p - i * W;
                  it.x = ld4(pcat + (static_cast<size_t>(i + 1) * Wp + (j + 1)) * ld + 4 * v);
-                 it.g = fold_read(gp, ld, 0, H, W, i, j, v);
+                 it.g = fold_read<ZP>(gp, ld, 0, H, W, i, j, v);
                  return it;
                },
                [&](int p, const RedItem& it) {
@@ -1001,17 +1028,19 @@ __device__ __forceinline__ void d_cat_bwd_apply(const float* __restrict__ pcat, 
                  st4(dcat + static_cast<size_t>(p) * C + 4 * v, dx);
                });
 }
+template <bool ZP>
 __global__ void __launch_bounds__(256) k_cat_bwd_apply(const float* __restrict__ pcat, BnRef bn_cat, const float* __restrict__ gp,
                                                        int ld, int H, int W, const double* __restrict__ bwd,
                                                        float* __restrict__ dcat, int VL, int PPB) {
   pdl_enter();
-  d_cat_bwd_apply(pcat, bn_cat, gp, ld, H, W, bwd, dcat, VL, PPB);
+  d_cat_bwd_apply<ZP>(pcat, bn_cat, gp, ld, H, W, bwd, dcat, VL, PPB);
 }
 void launch_cat_bwd_apply(const float* pcat, BnRef bn_cat, const float* gp, int ld, int H, int W, const double* bwd,
-                          float* dcat, cudaStream_t s) {
+                          float* dcat, cudaStream_t s, int zero_pad) {
   VecGeom g = vec_geom(bn_cat.C, static_cast<long long>(H) * W);
-  fit_grid(g, k_cat_bwd_apply, 0);
-  launch_k(k_cat_bwd_apply, dim3(g.blocks), dim3(g.threads), 0, s, 1, pcat, bn_cat, gp, ld, H, W, bwd, dcat, g.VL, g.PPB);
+  auto kernel = zero_pad ? k_cat_bwd_apply<true> : k_cat_bwd_apply<false>;
+  fit_grid(g, kernel, 0);
+  launch_k(kernel, dim3(g.blocks), dim3(g.threads), 0, s, 1, pcat, bn_cat, gp, ld, H, W, bwd, dcat, g.VL, g.PPB);
 }
 
 // Adjoint of the x2 upsampling, materialised once: dst[h][w][C] <- D[2h][2w][ld] (channels coff..coff+C)
@@ -1382,6 +1411,8 @@ void launch_noise(const float* z0, float* z, float sigma, uint64_t seed, uint64_
 // outputs of a block go to four consecutive x of one (channel, row).  Block = one source row x 32 source columns; phase 1:
 // thread (channel, group of 4 pixels) generates; phase 2: thread (channel, pixel) writes the interior position and every halo
 // position that mirrors it (ReflectionPad2d(1): padded row 0 <- source row 1, row H+1 <- row H-2, same for columns).
+// ZP (zero padding): the source pixels on the image border write zeros into the halo cells next to them instead.
+template <bool ZP>
 __global__ void __launch_bounds__(256) k_noise_pad(const float* __restrict__ z0, float sigma, uint64_t seed, uint64_t offset,
                                                    const int* __restrict__ it_dev, float* __restrict__ dst, int C, int H, int W,
                                                    int Cs, Twin t16) {
@@ -1428,8 +1459,8 @@ __global__ void __launch_bounds__(256) k_noise_pad(const float* __restrict__ z0,
     if (c0 + tx < C) {
       int rows[3], nr = 0;
       rows[nr++] = sy + 1;
-      if (sy == 1) rows[nr++] = 0;
-      if (sy == H - 2) rows[nr++] = H + 1;
+      if (sy == (ZP ? 0 : 1)) rows[nr++] = 0;
+      if (sy == (ZP ? H - 1 : H - 2)) rows[nr++] = H + 1;
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
         const int pix = ty + 8 * k, sx = x0 + pix;
@@ -1437,12 +1468,13 @@ __global__ void __launch_bounds__(256) k_noise_pad(const float* __restrict__ z0,
         const float o = tile[pix][tx];
         int cols[3], nc = 0;
         cols[nc++] = sx + 1;
-        if (sx == 1) cols[nc++] = 0;
-        if (sx == W - 2) cols[nc++] = W + 1;
+        if (sx == (ZP ? 0 : 1)) cols[nc++] = 0;
+        if (sx == (ZP ? W - 1 : W - 2)) cols[nc++] = W + 1;
         for (int a = 0; a < nr; ++a)
           for (int b = 0; b < nc; ++b) {
-            dst[(static_cast<size_t>(rows[a]) * Wp + cols[b]) * C + c0 + tx] = o;
-            if (t16.p != nullptr) t16.p[(static_cast<size_t>(rows[a]) * Wp + cols[b]) * t16.ld + c0 + tx] = bf16_bits(o);
+            const float ob = ZP && (a > 0 || b > 0) ? 0.f : o;
+            dst[(static_cast<size_t>(rows[a]) * Wp + cols[b]) * C + c0 + tx] = ob;
+            if (t16.p != nullptr) t16.p[(static_cast<size_t>(rows[a]) * Wp + cols[b]) * t16.ld + c0 + tx] = bf16_bits(ob);
           }
       }
     }
@@ -1450,9 +1482,10 @@ __global__ void __launch_bounds__(256) k_noise_pad(const float* __restrict__ z0,
   }
 }
 void launch_noise_pad(const float* z0, float sigma, uint64_t seed, uint64_t offset, const int* it_dev, float* dst, int C, int H,
-                      int W, int c_src, cudaStream_t s, Twin t16) {
+                      int W, int c_src, cudaStream_t s, Twin t16, int zero_pad) {
   dim3 grid((W + 31) / 32, H);
-  launch_k(k_noise_pad, dim3(grid), dim3(256), 0, s, 1, z0, sigma, seed, offset, it_dev, dst, C, H, W, c_src > 0 ? c_src : C, t16);
+  launch_k(zero_pad ? k_noise_pad<true> : k_noise_pad<false>, dim3(grid), dim3(256), 0, s, 1, z0, sigma, seed, offset, it_dev, dst,
+           C, H, W, c_src > 0 ? c_src : C, t16);
 }
 __global__ void k_advance(int* it) {
   pdl_enter(); it[0] += 1; it[1] += 1; }  // {global Adam step, iteration index of this call}

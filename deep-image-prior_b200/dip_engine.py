@@ -17,6 +17,9 @@ PRECISION_TF32 = 0
 PRECISION_FP32 = 1
 PRECISION_BF16 = 2
 
+PAD_REFLECTION = 0   # dip_plan_opts.pad_mode: nn.ReflectionPad2d(1) before every 3x3 conv (models.skip pad='reflection')
+PAD_ZERO = 1         # Conv2d(padding=1): every other value of models.skip's `pad` (reference: models/common.py:114-120)
+
 
 class NetDesc(ctypes.Structure):
     _fields_ = [
@@ -37,6 +40,11 @@ class NetDesc(ctypes.Structure):
     ]
 
 
+class PlanOpts(ctypes.Structure):
+    """dip_plan_opts (include/dip.h)"""
+    _fields_ = [("pad_mode", ctypes.c_int)]
+
+
 _lib = None
 
 # every symbol include/dip.h declares (checked by tests/test_abi.py)
@@ -47,7 +55,7 @@ ABI_SYMBOLS = [
     "dip_run_iterations", "dip_plan_buffer", "dip_plan_num_launches", "dip_plan_set_timing", "dip_plan_get_timing", "dip_plan_get_timing_records", "dip_op_scratch_bytes", "dip_op_conv_fprop",
     "dip_op_conv_dgrad", "dip_op_conv_wgrad", "dip_op_conv_dgrad_s2",
     "dip_lanczos_down_out_size", "dip_lanczos_down_fwd", "dip_lanczos_down_bwd", "dip_plan_set_downsampler",
-    "dip_input_grad",
+    "dip_input_grad", "dip_plan_workspace_bytes_opts", "dip_plan_create_opts",
 ]
 
 
@@ -80,6 +88,9 @@ def lib():
     L.dip_plan_workspace_bytes.restype = sz
     L.dip_plan_workspace_bytes.argtypes = [ctypes.POINTER(NetDesc), i32, i32]
     L.dip_plan_create.argtypes = [ctypes.POINTER(NetDesc), i32, i32, vp, sz, pvp]
+    L.dip_plan_workspace_bytes_opts.restype = sz
+    L.dip_plan_workspace_bytes_opts.argtypes = [ctypes.POINTER(NetDesc), i32, i32, ctypes.POINTER(PlanOpts)]
+    L.dip_plan_create_opts.argtypes = [ctypes.POINTER(NetDesc), i32, i32, ctypes.POINTER(PlanOpts), vp, sz, pvp]
     L.dip_plan_destroy.argtypes = [vp]
     L.dip_plan_destroy.restype = None
     L.dip_plan_num_params.argtypes = [vp]
@@ -142,10 +153,15 @@ class Plan:
 
     def __init__(self, in_channels, out_channels, num_scales, channels, skip_channels, bilinear, H, W,
                  precision=PRECISION_TF32, device=None, need_sigmoid=True, input_grad=False, channels_up=None,
-                 downsample_mode="stride"):
+                 downsample_mode="stride", pad="reflection"):
         """channels / skip_channels: one width for every scale, or per-scale sequences (num_channels_down / num_channels_skip
-        of models.skip; channels_up = num_channels_up, default = channels)."""
+        of models.skip; channels_up = num_channels_up, default = channels).  pad: 'reflection' or 'zero' (the padding of
+        every 3x3 conv)."""
         L = lib()
+        if pad not in ("reflection", "zero"):
+            raise ValueError("dip-b200: Plan(pad=...) must be 'reflection' or 'zero', not %r" % (pad,))
+        self.opts = PlanOpts(PAD_REFLECTION if pad == "reflection" else PAD_ZERO)
+        self.pad = pad
         per_scale = None
         if isinstance(channels, (list, tuple)) or isinstance(skip_channels, (list, tuple)) or channels_up is not None:
             as_list = lambda x: list(x) if isinstance(x, (list, tuple)) else [x] * num_scales   # noqa: E731
@@ -171,14 +187,15 @@ class Plan:
                 for i, x in enumerate(vals):
                     arr[i] = int(x)
         self.H, self.W = H, W
-        nbytes = L.dip_plan_workspace_bytes(ctypes.byref(self.desc), H, W)
+        nbytes = L.dip_plan_workspace_bytes_opts(ctypes.byref(self.desc), H, W, ctypes.byref(self.opts))
         if nbytes == 0:
             raise NotImplementedError("libdip: " + L.dip_last_error().decode())
         with torch.cuda.device(self.device):
             self.workspace = torch.empty(nbytes + 512, dtype=torch.uint8, device=self.device)
             base = (self.workspace.data_ptr() + 255) // 256 * 256
             h = ctypes.c_void_p()
-            check(L.dip_plan_create(ctypes.byref(self.desc), H, W, ctypes.c_void_p(base), nbytes, ctypes.byref(h)))
+            check(L.dip_plan_create_opts(ctypes.byref(self.desc), H, W, ctypes.byref(self.opts), ctypes.c_void_p(base), nbytes,
+                                         ctypes.byref(h)))
         self.h = h
         self.n_params = L.dip_plan_num_params(h)
         self.n_bn = L.dip_plan_num_bn(h)

@@ -104,13 +104,13 @@ class SkipNet(nn.Sequential):
         import dip_engine as de
         spec = self._dip_spec
         H, W = key[0], key[1]
-        pkey = (H, W, str(z.device), prec, key[4])
+        pkey = (H, W, str(z.device), prec, key[4], spec.get('pad', 'reflection'))
         plan = self._dip_plans.get(pkey)
         if plan is None:
             plan = de.Plan(spec['in_channels'], spec['out_channels'], spec['num_scales'], spec['channels'],
                            spec['skip_channels'], spec['bilinear'], H, W, precision=prec, device=z.device,
                            need_sigmoid=spec['need_sigmoid'], input_grad=key[4], channels_up=spec.get('channels_up'),
-                           downsample_mode=spec.get('downsample_mode', 'stride'))
+                           downsample_mode=spec.get('downsample_mode', 'stride'), pad=spec.get('pad', 'reflection'))
             self._dip_plans[pkey] = plan
         params = list(self.parameters())
         for p in params:
@@ -261,8 +261,6 @@ def skip(num_input_channels=2, num_output_channels=3,
         why = 'num_channels_skip must be 0 or 4 per scale (or 128 at every scale of a 128-wide network)'
     elif set(filter_size_down) != {3} or set(filter_size_up) != {3} or filter_skip_size != 1:
         why = 'filter sizes must be 3/3/1'
-    elif pad != 'reflection':
-        why = "pad must be 'reflection'"
     elif set(downsample_mode) not in ({'stride'}, {'avg'}):
         why = "downsample_mode must be 'stride' or 'avg' (at every scale)"
     elif act_fun != 'LeakyReLU':
@@ -280,6 +278,9 @@ def skip(num_input_channels=2, num_output_channels=3,
                              channels_up=None if uniform else list(num_channels_up),
                              skip_channels=num_channels_skip[0] if uniform else list(num_channels_skip),
                              need_sigmoid=bool(need_sigmoid), downsample_mode=downsample_mode[0],
+                             # models/common.py:conv: only pad == 'reflection' inserts ReflectionPad2d, any other value
+                             # is Conv2d(padding=(k-1)//2), i.e. zero padding
+                             pad='reflection' if pad == 'reflection' else 'zero',
                              bilinear=(upsample_mode[0] == 'bilinear' if len(set(upsample_mode)) == 1
                                        else [m == 'bilinear' for m in upsample_mode]))
     else:

@@ -62,6 +62,18 @@ int dip_version(void);
 size_t dip_plan_workspace_bytes(const dip_net_desc* desc, int H, int W);
 int dip_plan_create(const dip_net_desc* desc, int H, int W, void* workspace, size_t workspace_bytes,
                     dip_plan** out);
+
+/* Plan options beyond dip_net_desc.  pad_mode = the `pad` argument of models.skip (reference: models/common.py:114-120):
+ * DIP_PAD_REFLECTION inserts nn.ReflectionPad2d before every 3x3 conv; any other value of `pad` gives
+ * Conv2d(padding=1), i.e. DIP_PAD_ZERO.  Both modes need the same workspace.  Other values are rejected. */
+enum { DIP_PAD_REFLECTION = 0, DIP_PAD_ZERO = 1 };
+typedef struct {
+  int pad_mode;          /* DIP_PAD_*                                                                     */
+} dip_plan_opts;
+/* as dip_plan_workspace_bytes / dip_plan_create; opts may be NULL (= reflection padding, what the two calls above use) */
+size_t dip_plan_workspace_bytes_opts(const dip_net_desc* desc, int H, int W, const dip_plan_opts* opts);
+int dip_plan_create_opts(const dip_net_desc* desc, int H, int W, const dip_plan_opts* opts, void* workspace,
+                         size_t workspace_bytes, dip_plan** out);
 void dip_plan_destroy(dip_plan* plan);
 int dip_plan_num_params(const dip_plan* plan);
 int dip_plan_num_bn(const dip_plan* plan);
