@@ -865,7 +865,9 @@ static int build_plan(dip_plan* P, Arena& A) {
     }
     if (v.dS != nullptr && CS > 0) reg(pf + "dS", v.dS, v.H, v.W, v.Cin, v.Cin);   // (written by the skip conv's dgrad only)
     if (v.ZS != nullptr) reg(pf + "ZS", v.ZS, v.H, v.W, nd, nd);
-    if (v.dPin != nullptr) reg(pf + "dPin", v.dPin, v.H + 2, v.W + 2, v.Cin, v.Cin);
+    // (level 0: the input gradient conv writes the real input depth only; the stored depth's extra channels are never
+    // written, and k_input_grad never reads them)
+    if (v.dPin != nullptr) reg(pf + "dPin", v.dPin, v.H + 2, v.W + 2, v.Cin, v.Cin_act);
   }
   P->out_saved = A.get<float>((size_t)P->H * P->W * d.out_channels);
   P->zbuf = A.get<float>((size_t)P->H * P->W * d.in_channels);

@@ -1117,13 +1117,19 @@ __device__ __forceinline__ float4 skinny_wrow(const float* __restrict__ w, int n
 }
 
 // ------------------------------------------------------------------------------------------------ skinny 1x1 convs
-// VL = C/4 lanes per pixel (power of two <= 32); warp-shuffle reduction over the pixel's lanes.
+// VL = C/4 lanes per pixel, rounded up to a power of two VLp <= 32 so that a pixel's lanes are an aligned group of the warp
+// for the shuffle reduction (C = 24, 40, 48, ... : VL = 6, 10, 12, ...); lanes v >= VL hold zeros.
+__host__ __device__ __forceinline__ int skinny_lanes(int C) {
+  int vlp = 1;
+  while (vlp < C / 4) vlp <<= 1;
+  return vlp;
+}
 __device__ __forceinline__ void d_skinny_fwd_narrow(const float* __restrict__ x, int ldx, int x_rs, const float* __restrict__ w,
                                                     const float* __restrict__ b, int C, int N, int H, int W,
                                                     float* __restrict__ y, int mode, double* __restrict__ stats, int cw) {
-  const int VL = C / 4;
-  const int PPB = 256 / VL;
-  const int v = threadIdx.x % VL, slot = threadIdx.x / VL;
+  const int VL = C / 4, VLp = skinny_lanes(C);
+  const int PPB = 256 / VLp;
+  const int v = threadIdx.x % VLp, slot = threadIdx.x / VLp;
   const int npix = H * W;
   float4 wv[4];
   float bv[4];
@@ -1138,13 +1144,13 @@ __device__ __forceinline__ void d_skinny_fwd_narrow(const float* __restrict__ x,
   for (int t = 0; t < trips; ++t) {
     const int p = (t * gridDim.x + blockIdx.x) * PPB + slot;
     float acc[4] = {0.f, 0.f, 0.f, 0.f};
-    if (p < npix) {
+    if (p < npix && v < VL) {
       const int i = p / W, j = p - i * W;
       const float4 xv = ld4(x + (static_cast<size_t>(i) * x_rs + j) * ldx + 4 * v);
 #pragma unroll
       for (int n = 0; n < 4; ++n) acc[n] = f4dot(xv, wv[n]);
     }
-    for (int o = VL >> 1; o > 0; o >>= 1) {
+    for (int o = VLp >> 1; o > 0; o >>= 1) {
 #pragma unroll
       for (int n = 0; n < 4; ++n) acc[n] += __shfl_xor_sync(0xffffffffu, acc[n], o);
     }
@@ -1253,7 +1259,8 @@ __global__ void __launch_bounds__(256) k_skinny_fwd(const float* __restrict__ x,
 }
 void launch_skinny_fwd(const float* x, int ldx, int x_rs, const float* w, const float* b, int C, int N, int H,
                        int W, float* y, int mode, double* stats, cudaStream_t s, int cw) {
-  const int PPB = C >= 32 ? 64 : 256 / (C / 4);   // pixels per block and trip (wide path: 64 whatever the depth)
+  const bool wide = mode == 0 && (C == 32 || C == 64 || C == 128);
+  const int PPB = wide ? 64 : 256 / skinny_lanes(C);   // pixels per block and trip of the path d_skinny_fwd takes
   long long nb = (static_cast<long long>(H) * W + PPB - 1) / PPB;
   if (nb > kNumSms * 8) nb = kNumSms * 8;
   launch_red(k_skinny_fwd, static_cast<int>(nb), 256, 2 * 256 * sizeof(float4) + 2 * 4 * sizeof(double), s, x, ldx, x_rs, w, b, C, N, H, W,

@@ -410,10 +410,8 @@ def backward(cfg, params, src, mode, refs, dout, input_grad=False):
             dy, stride = rd.op(pf + "dRawF"), 1
         else:
             dy, stride = rd.op(pf + "dRaw_d1"), 2
-        if l > 0 or input_grad:
-            g, t = conv_dgrad(dy, rd.w(pf + "d1.w"), stride, mode)
-            pad = (0, stored_depth(cfg, l) - cin)
-            refs.put_conv(pf + "dPin", mode, F.pad(g, pad), F.pad(t, pad))
+        if l > 0 or input_grad:   # (level 0: the real input depth; the stored depth's extra channels get no gradient)
+            refs.put_conv(pf + "dPin", mode, *conv_dgrad(dy, rd.w(pf + "d1.w"), stride, mode))
         refs.put_conv("grad:" + pf + "d1.w", mode, *conv_wgrad(rd.op(pf + "Pin", cin), dy, (nd, cin, 3, 3), stride, mode))
     if input_grad:   # dL/d(net input), torch layout 1 x C x H x W
         g = fold(rd("L0.dPin"))[..., :cfg.in_channels]
