@@ -37,18 +37,22 @@ __host__ __device__ constexpr int round32(int n) { return (n + 31) & ~31; }
 __host__ __device__ constexpr int round1024(int n) { return (n + 1023) & ~1023; }
 
 // ------------------------------------------------------------------------------------------------ fprop / dgrad
+template <int NT>
+__device__ __forceinline__ void tc_conv_epilogue(const TcConvParams& p, const TcConvParams* pm, SmemCtl* ctl, uint8_t* staging,
+                                                 float (&acc)[2][NT / 2], int x0, int y0, int opx, int opy, int n_off,
+                                                 double& stat_s1, double& stat_s2, bool col_halves = false);
+__device__ __forceinline__ void tc_conv_stats_flush(const TcConvParams& p, int n_off, double stat_s1, double stat_s2);
+
 // Consumer warpgroup (threads 128..255) of the conv kernel, NT = wgmma N (n_mma rounded up to 32).
 template <bool BF16, int NT>
 __device__ __forceinline__ void tc_conv_consumer(const TcConvParams& p, const TcConvParams* pm, SmemCtl* ctl,
                                                  uint8_t* stage_base, int stage_bytes, uint8_t* staging, int n_iters,
                                                  int tile0, int tile_stride, int num_tiles, int tiles_pp, int n_off) {
-  const int et = threadIdx.x - 128;    // 0..127
-  const int w = et >> 5, lane = et & 31;
+  const int lane = threadIdx.x & 31;
   float acc[2][NT / 2];
   int stage = 0;
   uint32_t phase = 0;
   double stat_s1 = 0.0, stat_s2 = 0.0;
-  const int bw_shift = 31 - __clz(p.bw);  // tile widths are powers of two
   const uint32_t base_lo = desc_lo(smem_u32(stage_base));
   const uint32_t stage_step = static_cast<uint32_t>(stage_bytes) >> 4;
   constexpr uint32_t kBOff = static_cast<uint32_t>(kABytes) >> 4;
@@ -92,7 +96,21 @@ __device__ __forceinline__ void tc_conv_consumer(const TcConvParams& p, const Tc
     }
     wgmma_wait<0>();
     if (prev >= 0 && lane == 0) mbar_arrive(&ctl->empty[prev]);
+    tc_conv_epilogue<NT>(p, pm, ctl, staging, acc, x0, y0, opx, opy, n_off, stat_s1, stat_s2);
+  }
+  tc_conv_stats_flush(p, n_off, stat_s1, stat_s2);
+}
 
+// Epilogue of one tile (consumer warpgroup): + bias -> swizzled staging -> TMA store, and the tile's per-channel
+// statistics added to the running totals s1 / s2.
+template <int NT>
+__device__ __forceinline__ void tc_conv_epilogue(const TcConvParams& p, const TcConvParams* pm, SmemCtl* ctl, uint8_t* staging,
+                                                 float (&acc)[2][NT / 2], int x0, int y0, int opx, int opy, int n_off,
+                                                 double& stat_s1, double& stat_s2, bool col_halves) {
+  const int et = threadIdx.x - 128;    // 0..127
+  const int w = et >> 5, lane = et & 31;
+  const int bw_shift = 31 - __clz(p.bw);  // tile widths are powers of two
+  {
     // staging buffer must be free (previous tile's TMA store has finished reading it)
     if (et == 0) tma_store_wait_read0();
     named_bar_sync(1, 128);
@@ -106,7 +124,10 @@ __device__ __forceinline__ void tc_conv_consumer(const TcConvParams& p, const Tc
           const int q = (col & 31) >> 2, e = col & 3;
 #pragma unroll
           for (int rr = 0; rr < 2; ++rr) {
-            const int row = 64 * h + 16 * w + (lane >> 2) + 8 * rr;
+            // accumulator row -> staging row (pixel py * bw + px): the m64 halves are the tile's two row halves, or, for the
+            // 16-wide tiles of the patch path (col_halves), its two 8-pixel column halves
+            const int r64 = 16 * w + (lane >> 2) + 8 * rr;
+            const int row = col_halves ? ((r64 >> 3) << 4) + 8 * h + (r64 & 7) : 64 * h + r64;
             float2 o;
             o.x = acc[h][4 * j + 2 * rr] + ctl->bias[col];
             o.y = acc[h][4 * j + 2 * rr + 1] + ctl->bias[col + 1];
@@ -152,6 +173,11 @@ __device__ __forceinline__ void tc_conv_consumer(const TcConvParams& p, const Tc
       stat_s2 += static_cast<double>(b0 + b1);
     }
   }
+}
+
+// End of the consumer warpgroup's work: one fp64 atomic pair per channel, then wait for the last TMA store.
+__device__ __forceinline__ void tc_conv_stats_flush(const TcConvParams& p, int n_off, double stat_s1, double stat_s2) {
+  const int et = threadIdx.x - 128;
   if (p.stats != nullptr && et < p.n_mma && n_off + et < p.stats_ld) {
     const int rep = (blockIdx.x % kAccR) * kAccLine;
     atomicAdd(&p.stats[(n_off + et) * kAccStride + rep], stat_s1);
@@ -278,6 +304,207 @@ __global__ void __launch_bounds__(kNumThreads, 1) tc_conv_kernel(const __grid_co
 __global__ void __launch_bounds__(kNumThreads, 1) tc_conv_kernel_bf16(const __grid_constant__ TcConvParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   tc_conv_body<false, true>(p, &p, smem_raw);
+}
+
+// ------------------------------------------------------------------------------------------------ stride-1 3x3 patch path
+// tc_conv_patch_kernel: tc_conv_kernel for stride-1 3x3 convolutions (fprop and the stride-1 dgrad) on tiles 8 or 16
+// pixels wide, with the same tiles, warp roles, weight stages, wgmma sequence and epilogue -- only the activation operand
+// arrives differently.  Instead of one shifted 128-pixel tile per tap and K block, the producer loads, per tile and K
+// block, the (bh + 2) x (bw + 2) = 180 pixel input patch ONCE, and the nine taps read it at nine offsets.  All K blocks of
+// a tile stay resident (one patch slot per K block, each with its own pfull / pempty barrier), so the wgmmas run in
+// exactly tc_conv_kernel's order -- taps outer, K blocks inner -- and every accumulator receives the same sums in the same
+// order: the results are those of tc_conv_kernel, bit for bit.
+// Layout: TMA writes a patch unswizzled as [16-byte channel group][patch row][patch col][16 B], so a wgmma core matrix
+// (8 rows x 16 B) is 8 consecutive pixels of one patch row, contiguous at any pixel offset.  The two m64 halves of the
+// tile are eight 8-pixel segments at a constant stride of one patch row: the eight rows 8h .. 8h + 7 of an 8 x 16 tile,
+// or the eight rows of column half h (pixels 8h .. 8h + 7) of a 16 x 8 tile.  The A descriptor of tap (r, s), half h and
+// K step k is then
+//   start = patch + (r * PW + s + half_off(h)) * 16 B + k * 2 * plane,   SBO = PW * 16 B (one patch row),   LBO = plane
+// (PW = bw + 2, half_off = 8 PW h for bw = 8 and 8 h for bw = 16, plane = one channel group of the patch, kPatchPlane); the
+// epilogue maps accumulator rows back to staging rows py * bw + px.  The weights keep their 128-byte-swizzled stages.
+// L2 -> SM bytes per tile and K block: 22.5 KB of activation + 9 weight tiles, instead of 9 x (16 KB + weight tile).
+// wgmma N of the patch path: n_mma rounded up to 32, except 144 (the input gradient of the 128 + 4 channel concat convs,
+// 144 = 132 rounded up to 16), which would otherwise give 16 zero columns and 2 KB of every weight stage to rounding
+__host__ __device__ constexpr int patch_nt(int n_mma) { return n_mma == 144 ? 144 : round32(n_mma); }
+struct PatchCtl {
+  uint64_t pfull[kPatchMaxKb];
+  uint64_t pempty[kPatchMaxKb];
+};
+
+// Trip counts of one CTA, shared by the producer and the consumer (both walk tiles, then the 9 taps, then K blocks).
+struct PatchWork {
+  int tile0, tile_stride, n_iters, n_off, n_total;
+};
+__device__ __forceinline__ PatchWork patch_work(const TcConvParams& p) {
+  const int n_split = p.n_split < 1 ? 1 : p.n_split;
+  PatchWork w;
+  const int num_tiles = p.tiles_x * p.tiles_y;
+  w.tile_stride = static_cast<int>(gridDim.x) / n_split;
+  w.tile0 = blockIdx.x / n_split;
+  w.n_iters = (num_tiles - w.tile0 + w.tile_stride - 1) / w.tile_stride;   // tiles tile0, tile0 + stride, ... < num_tiles
+  w.n_off = static_cast<int>(blockIdx.x % n_split) * p.n_mma;
+  w.n_total = p.n_mma * n_split;
+  return w;
+}
+static constexpr int kPatchTaps = 9;
+
+template <bool BF16, int NT>
+__device__ __forceinline__ void tc_conv_patch_consumer(const TcConvParams& p, const TcConvParams* pm, SmemCtl* ctl, PatchCtl* pc,
+                                                       uint8_t* patch_base, uint8_t* b_base, int b_stage_bytes,
+                                                       uint8_t* staging, const PatchWork& wk) {
+  const int lane = threadIdx.x & 31;
+  float acc[2][NT / 2];
+  int stage = 0;
+  uint32_t phase = 0, pphase = 0;
+  double stat_s1 = 0.0, stat_s2 = 0.0;
+  const uint32_t patch16 = smem_u32(patch_base) >> 4;
+  const uint32_t b_lo0 = desc_lo(smem_u32(b_base));
+  const uint32_t b_step = static_cast<uint32_t>(b_stage_bytes) >> 4;
+  constexpr uint32_t kPlane16 = kPatchPlane >> 4, kSlot16 = kPatchBytes >> 4;
+  const uint32_t row16 = p.bw + 2;                              // one patch row, in 16-byte units
+  const uint32_t half16 = p.bw == 8 ? 8 * row16 : 8;            // second m64 half: 8 rows down, or 8 pixels right
+  for (int it = 0; it < wk.n_iters; ++it) {
+    const int tile = wk.tile0 + it * wk.tile_stride;
+    const int x0 = (tile % p.tiles_x) * p.bw, y0 = (tile / p.tiles_x) * p.bh;
+#pragma unroll
+    for (int i = 0; i < NT / 2; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
+    int prev = -1;         // B stage read by the previous wgmma group
+    int prev_patch = -1;   // patch slot read by the previous group if it was that slot's last (tap 8)
+#pragma unroll 1
+    for (int tap = 0; tap < kPatchTaps; ++tap) {
+      const int r = tap / 3, s = tap - 3 * (tap / 3);
+#pragma unroll 1
+      for (int kb = 0; kb < p.kblocks; ++kb) {
+        if (tap == 0) mbar_wait(&pc->pfull[kb], pphase);
+        mbar_wait(&ctl->full[stage], phase);
+        const uint32_t b_lo = b_lo0 + stage * b_step;
+        const uint32_t a16 = patch16 + kb * kSlot16 + r * row16 + s;
+        // all four K steps of every block, as in tc_conv_consumer (channels past the K extent are zero in both operands)
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          wgmma_ss<NT, BF16>(acc[0], desc_noswz(a16 + 2 * k * kPlane16, kPlane16, row16), desc_of(b_lo + 2 * k));
+          wgmma_ss<NT, BF16>(acc[1], desc_noswz(a16 + half16 + 2 * k * kPlane16, kPlane16, row16), desc_of(b_lo + 2 * k));
+        }
+        wgmma_commit();
+        if (prev >= 0) {   // the previous group's wgmmas have read their operands -> hand them back to the producer
+          wgmma_wait<1>();
+          if (lane == 0) {
+            mbar_arrive(&ctl->empty[prev]);
+            if (prev_patch >= 0) mbar_arrive(&pc->pempty[prev_patch]);
+          }
+        }
+        prev = stage;
+        prev_patch = tap == kPatchTaps - 1 ? kb : -1;
+        if (++stage == p.stages) { stage = 0; phase ^= 1; }
+      }
+    }
+    pphase ^= 1;
+    wgmma_wait<0>();
+    if (prev >= 0 && lane == 0) {
+      mbar_arrive(&ctl->empty[prev]);
+      if (prev_patch >= 0) mbar_arrive(&pc->pempty[prev_patch]);
+    }
+    tc_conv_epilogue<NT>(p, pm, ctl, staging, acc, x0, y0, 0, 0, wk.n_off, stat_s1, stat_s2, p.bw == 16);
+  }
+  tc_conv_stats_flush(p, wk.n_off, stat_s1, stat_s2);
+}
+
+template <bool BF16>
+__device__ __forceinline__ void tc_conv_patch_body(const TcConvParams& p, uint8_t* smem_raw) {
+  constexpr int KE = BF16 ? 64 : 32;   // channels per 128-byte operand row
+  constexpr int KG = BF16 ? 8 : 4;     // channels per 16-byte group
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  const int nt = patch_nt(p.n_mma);
+  const int b_bytes = p.n_mma * 128;
+  const int b_stage_bytes = round1024(nt * 128);
+  // layout: [B stages | epilogue staging | one patch per K block | control]; stages and staging 1024-byte aligned (swizzle
+  // atoms), patches 128-byte aligned (kPatchBytes is a multiple of 128)
+  uint8_t* b_base = smem;
+  uint8_t* staging = b_base + p.stages * b_stage_bytes;
+  uint8_t* patch_base = staging + p.n_chunks * kChunkBytes;
+  SmemCtl* ctl = reinterpret_cast<SmemCtl*>(patch_base + p.kblocks * kPatchBytes);
+  PatchCtl* pc = reinterpret_cast<PatchCtl*>(ctl + 1);
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const PatchWork wk = patch_work(p);
+
+  pdl_trigger();
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&p.tmA);
+    tma_prefetch_desc(&p.tmB);
+    tma_prefetch_desc(&p.tmD);
+  }
+  if (warp == 1 && lane == 0) {
+    for (int i = 0; i < p.stages; ++i) {
+      mbar_init(&ctl->full[i], 1);
+      mbar_init(&ctl->empty[i], 4);   // one arrival per consumer warp
+    }
+    for (int i = 0; i < p.kblocks; ++i) {
+      mbar_init(&pc->pfull[i], 1);
+      mbar_init(&pc->pempty[i], 4);
+    }
+    fence_mbar_init();
+  }
+  pdl_wait();
+  if (warp == 3) {
+    for (int i = lane; i < 160; i += 32)
+      ctl->bias[i] = (p.bias != nullptr && i < p.n_mma && (p.n_valid == 0 || wk.n_off + i < p.n_valid)) ? p.bias[wk.n_off + i] : 0.f;
+  }
+  __syncthreads();
+
+  if (warp == 0) {
+    // ===================================================================== TMA producer
+    // The whole warp walks the loop (warp-uniform control flow); one elected lane issues the TMA instructions.
+    int stage = 0;
+    uint32_t phase = 0, pphase = 0;
+    for (int it = 0; it < wk.n_iters; ++it) {
+      const int tile = wk.tile0 + it * wk.tile_stride;
+      const int x0 = (tile % p.tiles_x) * p.bw, y0 = (tile / p.tiles_x) * p.bh;
+      for (int tap = 0; tap < kPatchTaps; ++tap) {
+        for (int kb = 0; kb < p.kblocks; ++kb) {
+          if (tap == 0) {
+            // patch slot kb is free once the previous tile's last tap has read it
+            mbar_wait(&pc->pempty[kb], pphase ^ 1);
+            if (elect_one()) {
+              // out-of-range pixels (image border, dgrad's negative offsets, ragged tiles) and channels past C arrive as zeros
+              mbar_expect_tx(&pc->pfull[kb], kPatchBytes);
+              tma_load_4d(patch_base + kb * kPatchBytes, &p.tmA, &pc->pfull[kb], 0, x0 + p.offx, y0 + p.offy, kb * (KE / KG));
+            }
+            __syncwarp();
+          }
+          mbar_wait(&ctl->empty[stage], phase ^ 1);
+          if (elect_one()) {
+            mbar_expect_tx(&ctl->full[stage], b_bytes);
+            tma_load_2d(b_base + stage * b_stage_bytes, &p.tmB, &ctl->full[stage], kb * KE, tap * wk.n_total + wk.n_off);
+          }
+          __syncwarp();
+          if (++stage == p.stages) { stage = 0; phase ^= 1; }
+        }
+      }
+      pphase ^= 1;
+    }
+  } else if (warp >= 4) {
+    // ===================================================================== wgmma + epilogue (one warpgroup)
+    switch (nt) {
+      case 32: tc_conv_patch_consumer<BF16, 32>(p, &p, ctl, pc, patch_base, b_base, b_stage_bytes, staging, wk); break;
+      case 64: tc_conv_patch_consumer<BF16, 64>(p, &p, ctl, pc, patch_base, b_base, b_stage_bytes, staging, wk); break;
+      case 96: tc_conv_patch_consumer<BF16, 96>(p, &p, ctl, pc, patch_base, b_base, b_stage_bytes, staging, wk); break;
+      case 128: tc_conv_patch_consumer<BF16, 128>(p, &p, ctl, pc, patch_base, b_base, b_stage_bytes, staging, wk); break;
+      case 144: tc_conv_patch_consumer<BF16, 144>(p, &p, ctl, pc, patch_base, b_base, b_stage_bytes, staging, wk); break;
+      default: tc_conv_patch_consumer<BF16, 160>(p, &p, ctl, pc, patch_base, b_base, b_stage_bytes, staging, wk); break;
+    }
+  }
+  __syncthreads();
+}
+__global__ void __launch_bounds__(kNumThreads, 1) tc_conv_patch_kernel(const __grid_constant__ TcConvParams p) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  tc_conv_patch_body<false>(p, smem_raw);
+}
+__global__ void __launch_bounds__(kNumThreads, 1) tc_conv_patch_kernel_bf16(const __grid_constant__ TcConvParams p) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  tc_conv_patch_body<true>(p, smem_raw);
 }
 
 // ------------------------------------------------------------------------------------------------ wgrad
@@ -652,7 +879,10 @@ __global__ void __launch_bounds__(kNumThreads, 1) tc_wgrad_kernel_bf16(const __g
 static constexpr size_t kMaxSmem = 232448;  // 227 KB
 
 size_t tc_conv_smem_bytes(const TcConvParams& p) {
-  const size_t b_bytes = round1024(round32(p.n_mma) * 128);
+  const size_t b_bytes = round1024((p.patch ? patch_nt(p.n_mma) : round32(p.n_mma)) * 128);
+  if (p.patch)
+    return 1024 + p.stages * b_bytes + static_cast<size_t>(p.n_chunks) * kChunkBytes +
+           static_cast<size_t>(p.kblocks) * kPatchBytes + sizeof(SmemCtl) + sizeof(PatchCtl);
   return 1024 + p.stages * (kABytes + b_bytes) + static_cast<size_t>(p.n_chunks) * kChunkBytes + sizeof(SmemCtl);
 }
 size_t tc_wgrad_smem_bytes(const TcWgradParams& p) {
@@ -666,6 +896,10 @@ cudaError_t tc_kernels_init() {
   if (e != cudaSuccess) return e;
   e = cudaFuncSetAttribute(tc_conv_kernel_bf16, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxSmem);
   if (e != cudaSuccess) return e;
+  e = cudaFuncSetAttribute(tc_conv_patch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxSmem);
+  if (e != cudaSuccess) return e;
+  e = cudaFuncSetAttribute(tc_conv_patch_kernel_bf16, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxSmem);
+  if (e != cudaSuccess) return e;
   e = cudaFuncSetAttribute(tc_wgrad_kernel_bf16, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxSmem);
   if (e != cudaSuccess) return e;
   return cudaFuncSetAttribute(tc_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxSmem);
@@ -674,7 +908,8 @@ cudaError_t tc_kernels_init() {
 static bool conv_params_ok(const TcConvParams& p) {
   return p.n_mma >= 1 && p.n_mma <= 160 && p.n_chunks == (p.n_mma + 31) / 32 && p.stages >= 1 && p.stages <= 8 &&
          p.kblocks >= 1 && p.nphase >= 0 && p.nphase <= 4 &&
-         (p.bw & (p.bw - 1)) == 0 && p.bw * p.bh == kTileM;
+         (p.bw & (p.bw - 1)) == 0 && p.bw * p.bh == kTileM &&
+         (!p.patch || (((p.bw == 8 && p.bh == 16) || (p.bw == 16 && p.bh == 8)) && p.kblocks <= kPatchMaxKb && p.kh == 3 && p.kw == 3 && p.stride == 1 && p.nphase == 0));
 }
 
 cudaError_t tc_conv_launch(const TcConvParams& p, int num_sms, cudaStream_t s) {
@@ -687,6 +922,8 @@ cudaError_t tc_conv_launch(const TcConvParams& p, int num_sms, cudaStream_t s) {
   }
   const size_t smem = tc_conv_smem_bytes(p);
   if (smem > kMaxSmem) return cudaErrorInvalidValue;
+  if (p.patch)
+    return launch_k(p.bf16 ? tc_conv_patch_kernel_bf16 : tc_conv_patch_kernel, dim3(grid), dim3(kNumThreads), smem, s, 1, p);
   return launch_k(p.bf16 ? tc_conv_kernel_bf16 : tc_conv_kernel, dim3(grid), dim3(kNumThreads), smem, s, 1, p);
 }
 // grid the stand-alone launch uses (the persistent deep-level kernel runs the same CTA -> tile mapping on its first vgrid CTAs)

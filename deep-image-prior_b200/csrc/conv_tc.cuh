@@ -40,7 +40,15 @@ struct TcConvParams {
   const float* bias;       // [n_valid] or nullptr
   double* stats;           // [2][stats_ld] per-channel sum / sum of squares (fp64 atomics) or nullptr
   int stats_ld;
+  // patch = 1: the stride-1 3x3 path (tc_conv_patch_kernel), tiles bw x bh = 8 x 16 or 16 x 8.  Per tile and K block one
+  // (bh + 2) x (bw + 2) pixel patch feeds all nine taps.  tmA is then the 4-D map (channels of one 16-byte group, X, Y,
+  // group) of the activation with box {group, bw + 2, bh + 2, 8}: TMA writes the patch as [group][patch row][patch col][16 B].
+  int patch;
 };
+// geometry of the patch path (tc_conv_patch_kernel)
+static constexpr int kPatchPlane = 180 * 16;   // one 16-byte channel group of a (bh + 2) x (bw + 2) = 180 pixel patch (2880 B)
+static constexpr int kPatchMaxKb = 8;          // K blocks (resident patches) per tile at most
+static constexpr int kPatchBytes = 8 * kPatchPlane;                    // one K block: 128 bytes per pixel (23040 B)
 
 // Weight-gradient GEMM:  dW[tap][n][c] = sum_{pixels} dY[pixel][n] * X[pixel (+) tap][c]
 //   dY : NHWC [H][W][N] (fp32 or bf16 twin; N <= 128 output channels, channels >= N read as zero) through a 3-D map (N, W, H)

@@ -70,10 +70,10 @@ static int engine_init() {
 static bool is_tc(int prec) { return prec == DIP_PRECISION_TF32 || prec == DIP_PRECISION_BF16; }   // tensor-core paths
 
 static int encode_map(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_b,
-                      const cuuint32_t* box, bool bf16 = false) {
+                      const cuuint32_t* box, bool bf16 = false, bool swizzle = true) {
   cuuint32_t estr[5] = {1, 1, 1, 1, 1};
   CUresult r = g_encode(m, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, rank, const_cast<void*>(base), dims, strides_b, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                        CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -107,6 +107,17 @@ static int map_act3(CUtensorMap* m, const void* base, int rows, int cols, int ld
   cuuint64_t str[2] = {ld * e, (cuuint64_t)cols * ld * e};
   cuuint32_t box[3] = {bf16 ? 64u : 32u, (cuuint32_t)bw, (cuuint32_t)bh};
   return encode_map(m, base, 3, dims, str, box, bf16);
+}
+// activation [rows][cols][ld] (c valid channels, a multiple of the 16-byte group) as the 4-D view (channels of one 16-byte
+// group, X, Y, group) read by the patch path of the conv kernel: one box {group, bw + 2, bh + 2, 8 groups} is the input
+// patch of one bw x bh tile and 128-byte K block, written unswizzled as [group][patch row][patch col][16 B]
+static int map_patch(CUtensorMap* m, const void* base, int rows, int cols, int ld, int c, int bw, int bh, bool bf16) {
+  const cuuint64_t e = bf16 ? 2 : sizeof(float);
+  const cuuint64_t g = 16 / e;
+  cuuint64_t dims[4] = {g, (cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)c / g};
+  cuuint64_t str[3] = {ld * e, (cuuint64_t)cols * ld * e, 16};
+  cuuint32_t box[4] = {(cuuint32_t)g, (cuuint32_t)bw + 2, (cuuint32_t)bh + 2, 8};
+  return encode_map(m, base, 4, dims, str, box, bf16, false);
 }
 static int map_w2(CUtensorMap* m, const void* base, int rows_total, int kcols, int box_rows, bool bf16 = false) {
   const cuuint64_t e = bf16 ? 2 : sizeof(float);
@@ -172,7 +183,7 @@ static int pick_nsplit(int tiles, int n_rows) {
   return sp;
 }
 static void fit_stages(TcConvParams& p, size_t budget = 232448) {
-  p.stages = 6;
+  p.stages = p.patch ? 8 : 6;
   while (tc_conv_smem_bytes(p) > budget && p.stages > 2) p.stages--;
 }
 struct ConvOp {
@@ -214,7 +225,8 @@ struct ConvOp {
   const float* wg_dy = nullptr; int wg_h = 0, wg_w = 0;
   // param slots
   int p_w = -1, p_b = -1;
-  TcConvParams fp{}, dg{};
+  TcConvParams fp{}, dg{};   // the general path (also the persistent deep-level kernel's ops)
+  TcConvParams fp_run{}, dg_run{};   // what the stand-alone launches run: fp / dg, or their stride-1 3x3 patch form
   TcWgradParams wg{};
   int simt_ksplits = 1;
 
@@ -245,6 +257,22 @@ struct ConvOp {
     return is_tc(prec) ? wacc_elems() : (size_t)simt_ksplits * k * k * 128 * c_pad;
   }
 
+  // The patch form q of a stride-1 3x3 conv g of the general path (tc_conv_patch_kernel): the same tiles, weights, output
+  // and N split, the activation [rows][cols][ld] (kc K channels) through the 4-D patch map.  It applies when the tile is 8
+  // or 16 pixels wide, the K channels fill whole 16-byte groups (TMA zero-fills the patch past the channel extent only in
+  // whole groups) and one patch per K block fits in shared memory beside at least two weight stages; otherwise q = g.  Both
+  // forms compute the same sums in the same order.  The persistent deep-level kernel always runs the general form.
+  int patch_form(const TcConvParams& g, TcConvParams& q, const void* act, int rows, int cols, int ld, int kc) {
+    q = g;
+    if ((g.bw != 8 && g.bw != 16) || kc % (bf16 ? 8 : 4) != 0 || g.kblocks > kPatchMaxKb) return 0;
+    TcConvParams t = g;
+    t.patch = 1;
+    fit_stages(t);
+    if (tc_conv_smem_bytes(t) > 232448) return 0;
+    DIP_CHECK(map_patch(&t.tmA, act, rows, cols, ld, kc, g.bw, g.bh, bf16));
+    q = t;
+    return 0;
+  }
   int build_tc(float* partial) {
     // ---- fprop
     int bw, bh;
@@ -266,6 +294,9 @@ struct ConvOp {
     fp.bias = nullptr; fp.stats = stats; fp.stats_ld = N;
     fit_stages(fp);
     }
+    fp_run = fp;
+    if (do_fprop && k == 3 && stride == 1)
+      DIP_CHECK(bf16 ? patch_form(fp, fp_run, in16, in_rows, in_cols, in_ld16, C) : patch_form(fp, fp_run, in, in_rows, in_cols, in_ld, C));
     // ---- dgrad
     if (has_dgrad && dg_s2) {
       // phase grid: (dg_out_h / 2) x (dg_out_w / 2) positions per parity class of the padded gradient
@@ -310,6 +341,9 @@ struct ConvOp {
       dg.bias = nullptr; dg.stats = nullptr; dg.stats_ld = 0;
       fit_stages(dg);
     }
+    dg_run = dg;
+    if (has_dgrad && !dg_s2 && k == 3)
+      DIP_CHECK(bf16 ? patch_form(dg, dg_run, dg_in16, dg_in_h, dg_in_w, N, N) : patch_form(dg, dg_run, dg_in, dg_in_h, dg_in_w, N, N));
     // ---- wgrad
     wg = TcWgradParams{};
     if (!do_wgrad) return 0;
@@ -336,7 +370,7 @@ struct ConvOp {
 
   int run_fprop(int prec, const float* bias, cudaStream_t s) {
     if (is_tc(prec)) {
-      TcConvParams p = fp;
+      TcConvParams p = fp_run;
       p.bias = bias;
       TimeScope ts(timer, 0, alg_flops(), s);
       DIP_CUDA(tc_conv_launch(p, g_num_sms, s));
@@ -355,7 +389,7 @@ struct ConvOp {
   int run_dgrad(int prec, cudaStream_t s) {
     if (is_tc(prec)) {
       TimeScope ts(timer, 1, alg_flops(), s);
-      DIP_CUDA(tc_conv_launch(dg, g_num_sms, s));
+      DIP_CUDA(tc_conv_launch(dg_run, g_num_sms, s));
     } else {
       SimtConvArgs a{};
       a.A = dg_in; a.a_h = dg_in_h; a.a_w = dg_in_w; a.a_ld = N; a.a_c = N;

@@ -86,6 +86,14 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uin
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+__device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                            int c2, int c3) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes "
+      "[%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(dst)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
 __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
                                             int c2, int c3, int c4) {
   asm volatile(
@@ -130,6 +138,16 @@ __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sy
 __device__ __forceinline__ uint32_t desc_lo(uint32_t saddr) { return ((saddr >> 4) & 0x3FFFu) | (1u << 16); }
 static constexpr uint32_t kDescHiSw128 = (1024u >> 4) | (1u << 30);
 __device__ __forceinline__ uint64_t desc_of(uint32_t lo) { return (static_cast<uint64_t>(kDescHiSw128) << 32) | lo; }
+
+// Descriptor of a K-major operand WITHOUT swizzle (layout type 0).  A core matrix is 8 rows x 16 bytes, stored as 128
+// contiguous bytes; the canonical layout is ((8, m), (16 B, 2)) : ((16 B, SBO), (1, LBO)) -- LBO is the byte distance
+// between the two core matrices of one wgmma K step (along K), SBO the distance between 8-row groups (along M / N).
+// Start, LBO and SBO only need 16-byte alignment, so a start may move by any whole number of 16-byte rows.
+//   start16: start address >> 4;  lbo16 / sbo16: offsets >> 4
+__host__ __device__ constexpr uint64_t desc_noswz(uint32_t start16, uint32_t lbo16, uint32_t sbo16) {
+  return static_cast<uint64_t>(start16 & 0x3FFFu) | (static_cast<uint64_t>(lbo16 & 0x3FFFu) << 16) |
+         (static_cast<uint64_t>(sbo16 & 0x3FFFu) << 32);
+}
 
 
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {

@@ -1,7 +1,7 @@
 """Small-shape launches of every hand-written mbarrier / TMA / wgmma kernel for compute-sanitizer (SURVEY.md 5, 7.3.3):
   compute-sanitizer --tool memcheck|racecheck|synccheck python scripts/sanitize_ops.py
 Covers tc_conv_kernel (1x1, 3x3, stride 2, N split, K tail with C=132, several waves of ragged tiles, 4-phase stride-2
-dgrad), tc_wgrad_kernel (split-K partials, in-smem operand transpose) and one full forward + backward + Adam step of the
+dgrad), tc_conv_patch_kernel (stride-1 3x3: ragged tiles, one tile, N split 2 and 4, K tail), tc_wgrad_kernel (split-K partials, in-smem operand transpose) and one full forward + backward + Adam step of the
 engine at 64x64.  Without the sanitizer it runs as a plain parity check (relative errors vs torch-CPU fp64).
 DIP_SAN_PREC=2 runs the same launches in the bf16 mode (tc_conv_kernel_bf16 / tc_wgrad_kernel_bf16, bf16 twins written by the
 producer kernels); DIP_SAN_NARROW=1 adds a step of the per-scale-width network (snail) with 'avg' downsampling."""
@@ -25,8 +25,10 @@ def rel(a, b):
 
 PREC = int(os.environ.get("DIP_SAN_PREC", "0"))
 g = torch.Generator().manual_seed(0)
-# (C, k, stride, oh, ow): 1x1, 3x3 (N split), stride 2, K tail (C=132), several waves of ragged tiles
-for C, k, stride, oh, ow in [(128, 1, 1, 32, 32), (128, 3, 1, 16, 16), (32, 3, 2, 32, 32), (132, 3, 1, 40, 24), (128, 3, 1, 270, 150)]:
+# (C, k, stride, oh, ow): 1x1, 3x3 (N split), stride 2, K tail (C=132), several waves of ragged tiles; stride-1 3x3 patch
+# path: ragged 8x16 tiles, a single tile (N split 4), N split 2, K tail with ragged tiles
+for C, k, stride, oh, ow in [(128, 1, 1, 32, 32), (128, 3, 1, 16, 16), (32, 3, 2, 32, 32), (132, 3, 1, 40, 24), (128, 3, 1, 270, 150),
+                             (128, 3, 1, 37, 21), (128, 3, 1, 16, 8), (128, 3, 1, 80, 80), (132, 3, 1, 45, 30)]:
     ih, iw = (oh - 1) * stride + k, (ow - 1) * stride + k
     ih += ih % 2 if stride == 2 else 0
     iw += iw % 2 if stride == 2 else 0
