@@ -38,14 +38,14 @@ __host__ __device__ constexpr int round1024(int n) { return (n + 1023) & ~1023; 
 
 // ------------------------------------------------------------------------------------------------ fprop / dgrad
 template <int NT>
-__device__ __forceinline__ void tc_conv_epilogue(const TcConvParams& p, const TcConvParams* pm, SmemCtl* ctl, uint8_t* staging,
+__device__ __forceinline__ void tc_conv_epilogue(const TcConvParams& p, SmemCtl* ctl, uint8_t* staging,
                                                  float (&acc)[2][NT / 2], int x0, int y0, int opx, int opy, int n_off,
                                                  double& stat_s1, double& stat_s2, bool col_halves = false);
 __device__ __forceinline__ void tc_conv_stats_flush(const TcConvParams& p, int n_off, double stat_s1, double stat_s2);
 
 // Consumer warpgroup (threads 128..255) of the conv kernel, NT = wgmma N (n_mma rounded up to 32).
 template <bool BF16, int NT>
-__device__ __forceinline__ void tc_conv_consumer(const TcConvParams& p, const TcConvParams* pm, SmemCtl* ctl,
+__device__ __forceinline__ void tc_conv_consumer(const TcConvParams& p, SmemCtl* ctl,
                                                  uint8_t* stage_base, int stage_bytes, uint8_t* staging, int n_iters,
                                                  int tile0, int tile_stride, int num_tiles, int tiles_pp, int n_off) {
   const int lane = threadIdx.x & 31;
@@ -96,7 +96,7 @@ __device__ __forceinline__ void tc_conv_consumer(const TcConvParams& p, const Tc
     }
     wgmma_wait<0>();
     if (prev >= 0 && lane == 0) mbar_arrive(&ctl->empty[prev]);
-    tc_conv_epilogue<NT>(p, pm, ctl, staging, acc, x0, y0, opx, opy, n_off, stat_s1, stat_s2);
+    tc_conv_epilogue<NT>(p, ctl, staging, acc, x0, y0, opx, opy, n_off, stat_s1, stat_s2);
   }
   tc_conv_stats_flush(p, n_off, stat_s1, stat_s2);
 }
@@ -104,7 +104,7 @@ __device__ __forceinline__ void tc_conv_consumer(const TcConvParams& p, const Tc
 // Epilogue of one tile (consumer warpgroup): + bias -> swizzled staging -> TMA store, and the tile's per-channel
 // statistics added to the running totals s1 / s2.
 template <int NT>
-__device__ __forceinline__ void tc_conv_epilogue(const TcConvParams& p, const TcConvParams* pm, SmemCtl* ctl, uint8_t* staging,
+__device__ __forceinline__ void tc_conv_epilogue(const TcConvParams& p, SmemCtl* ctl, uint8_t* staging,
                                                  float (&acc)[2][NT / 2], int x0, int y0, int opx, int opy, int n_off,
                                                  double& stat_s1, double& stat_s2, bool col_halves) {
   const int et = threadIdx.x - 128;    // 0..127
@@ -140,9 +140,9 @@ __device__ __forceinline__ void tc_conv_epilogue(const TcConvParams& p, const Tc
     named_bar_sync(1, 128);
     if (et == 0) {
       if (p.nphase > 0)
-        for (int j = 0; j < p.n_chunks; ++j) tma_store_5d(&pm->tmD, staging + j * kChunkBytes, n_off + j * 32, opx, x0, opy, y0);
+        for (int j = 0; j < p.n_chunks; ++j) tma_store_5d(&p.tmD, staging + j * kChunkBytes, n_off + j * 32, opx, x0, opy, y0);
       else
-        for (int j = 0; j < p.n_chunks; ++j) tma_store_3d(&pm->tmD, staging + j * kChunkBytes, n_off + j * 32, x0, y0);
+        for (int j = 0; j < p.n_chunks; ++j) tma_store_3d(&p.tmD, staging + j * kChunkBytes, n_off + j * 32, x0, y0);
       tma_store_commit();
     }
     if (p.stats != nullptr && et < p.n_mma) {
@@ -186,18 +186,12 @@ __device__ __forceinline__ void tc_conv_stats_flush(const TcConvParams& p, int n
   if (et == 0) tma_store_wait_all0();
 }
 
-// Body of the conv kernel.  DEEP = false: the stand-alone launch (tc_conv_kernel).  DEEP = true: one PHASE of the persistent
-// deep-level kernel (deep.cu): `p` is a shared-memory copy of the scalars, `pm` the parameter block in global memory whose
-// tensor maps TMA reads; the CTA-local barriers are re-initialised here (every barrier of the previous phase has completed
-// all its phases by then); CTAs beyond the grid the stand-alone launch would have used (p.vgrid) sit the phase out.
-// BF16 = true: operands are bf16 (K = 16 per wgmma).  The BYTE geometry is unchanged -- an operand row is still 128 bytes,
-// now 64 channels, and one wgmma still advances 32 bytes along K -- so a "k block" is 64 channels, p.kblocks counts
-// those, and only the channel coordinate of the TMA boxes and the instruction type differ.
-template <bool DEEP, bool BF16 = false>
-__device__ __forceinline__ void tc_conv_body(const TcConvParams& p, const TcConvParams* pm, uint8_t* smem_raw) {
+// Body of the conv kernel.  BF16 = true: operands are bf16 (K = 16 per wgmma).  The BYTE geometry is unchanged -- an operand
+// row is still 128 bytes, now 64 channels, and one wgmma still advances 32 bytes along K -- so a "k block" is 64 channels,
+// p.kblocks counts those, and only the channel coordinate of the TMA boxes and the instruction type differ.
+template <bool BF16>
+__device__ __forceinline__ void tc_conv_body(const TcConvParams& p, uint8_t* smem_raw) {
   constexpr int KE = BF16 ? 64 : 32;   // channels per 128-byte operand row
-  const int grid_x = DEEP ? p.vgrid : static_cast<int>(gridDim.x);
-  if (DEEP && static_cast<int>(blockIdx.x) >= grid_x) return;
   // 1024-byte alignment is required by the 128B swizzle atoms.
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int nt = round32(p.n_mma);
@@ -219,15 +213,15 @@ __device__ __forceinline__ void tc_conv_body(const TcConvParams& p, const TcConv
   const int n_part = blockIdx.x % n_split;
   const int n_off = n_part * p.n_mma;             // first output channel of this CTA
   const int n_total = p.n_mma * n_split;          // rows per tap of the packed weights
-  const int tile_stride = grid_x / n_split;
+  const int tile_stride = static_cast<int>(gridDim.x) / n_split;
   const int n_iters = (num_tiles + tile_stride - 1) / tile_stride;
   const int tile0 = blockIdx.x / n_split;         // first tile; stride tile_stride
 
-  if (!DEEP) pdl_trigger();
+  pdl_trigger();
   if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&pm->tmA);
-    tma_prefetch_desc(&pm->tmB);
-    tma_prefetch_desc(&pm->tmD);
+    tma_prefetch_desc(&p.tmA);
+    tma_prefetch_desc(&p.tmB);
+    tma_prefetch_desc(&p.tmD);
   }
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < p.stages; ++i) {
@@ -236,7 +230,7 @@ __device__ __forceinline__ void tc_conv_body(const TcConvParams& p, const TcConv
     }
     fence_mbar_init();
   }
-  if (!DEEP) pdl_wait();  // everything above is independent of the previous kernel's results
+  pdl_wait();  // everything above is independent of the previous kernel's results
   if (warp == 3) {
     for (int i = lane; i < 160; i += 32)
       ctl->bias[i] = (p.bias != nullptr && i < p.n_mma && (p.n_valid == 0 || n_off + i < p.n_valid)) ? p.bias[n_off + i] : 0.f;
@@ -276,8 +270,8 @@ __device__ __forceinline__ void tc_conv_body(const TcConvParams& p, const TcConv
             uint8_t* sa = stage_base + stage * stage_bytes;
             if (elect_one()) {
               mbar_expect_tx(&ctl->full[stage], kABytes + b_bytes);
-              tma_load_5d(sa, &pm->tmA, &ctl->full[stage], kb * KE, cpx, cx, cpy, cy);
-              tma_load_2d(sa + kABytes, &pm->tmB, &ctl->full[stage], kb * KE, tap * n_total + n_off);
+              tma_load_5d(sa, &p.tmA, &ctl->full[stage], kb * KE, cpx, cx, cpy, cy);
+              tma_load_2d(sa + kABytes, &p.tmB, &ctl->full[stage], kb * KE, tap * n_total + n_off);
             }
             __syncwarp();
             if (++stage == p.stages) { stage = 0; phase ^= 1; }
@@ -288,22 +282,22 @@ __device__ __forceinline__ void tc_conv_body(const TcConvParams& p, const TcConv
   } else if (warp >= 4) {
     // ===================================================================== wgmma + epilogue (one warpgroup)
     switch (nt) {
-      case 32: tc_conv_consumer<BF16, 32>(p, pm, ctl, stage_base, stage_bytes, staging, n_iters, tile0, tile_stride, num_tiles, tiles_pp, n_off); break;
-      case 64: tc_conv_consumer<BF16, 64>(p, pm, ctl, stage_base, stage_bytes, staging, n_iters, tile0, tile_stride, num_tiles, tiles_pp, n_off); break;
-      case 96: tc_conv_consumer<BF16, 96>(p, pm, ctl, stage_base, stage_bytes, staging, n_iters, tile0, tile_stride, num_tiles, tiles_pp, n_off); break;
-      case 128: tc_conv_consumer<BF16, 128>(p, pm, ctl, stage_base, stage_bytes, staging, n_iters, tile0, tile_stride, num_tiles, tiles_pp, n_off); break;
-      default: tc_conv_consumer<BF16, 160>(p, pm, ctl, stage_base, stage_bytes, staging, n_iters, tile0, tile_stride, num_tiles, tiles_pp, n_off); break;
+      case 32: tc_conv_consumer<BF16, 32>(p, ctl, stage_base, stage_bytes, staging, n_iters, tile0, tile_stride, num_tiles, tiles_pp, n_off); break;
+      case 64: tc_conv_consumer<BF16, 64>(p, ctl, stage_base, stage_bytes, staging, n_iters, tile0, tile_stride, num_tiles, tiles_pp, n_off); break;
+      case 96: tc_conv_consumer<BF16, 96>(p, ctl, stage_base, stage_bytes, staging, n_iters, tile0, tile_stride, num_tiles, tiles_pp, n_off); break;
+      case 128: tc_conv_consumer<BF16, 128>(p, ctl, stage_base, stage_bytes, staging, n_iters, tile0, tile_stride, num_tiles, tiles_pp, n_off); break;
+      default: tc_conv_consumer<BF16, 160>(p, ctl, stage_base, stage_bytes, staging, n_iters, tile0, tile_stride, num_tiles, tiles_pp, n_off); break;
     }
   }
   __syncthreads();
 }
 __global__ void __launch_bounds__(kNumThreads, 1) tc_conv_kernel(const __grid_constant__ TcConvParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  tc_conv_body<false>(p, &p, smem_raw);
+  tc_conv_body<false>(p, smem_raw);
 }
 __global__ void __launch_bounds__(kNumThreads, 1) tc_conv_kernel_bf16(const __grid_constant__ TcConvParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  tc_conv_body<false, true>(p, &p, smem_raw);
+  tc_conv_body<true>(p, smem_raw);
 }
 
 // ------------------------------------------------------------------------------------------------ stride-1 3x3 patch path
@@ -349,7 +343,7 @@ __device__ __forceinline__ PatchWork patch_work(const TcConvParams& p) {
 static constexpr int kPatchTaps = 9;
 
 template <bool BF16, int NT>
-__device__ __forceinline__ void tc_conv_patch_consumer(const TcConvParams& p, const TcConvParams* pm, SmemCtl* ctl, PatchCtl* pc,
+__device__ __forceinline__ void tc_conv_patch_consumer(const TcConvParams& p, SmemCtl* ctl, PatchCtl* pc,
                                                        uint8_t* patch_base, uint8_t* b_base, int b_stage_bytes,
                                                        uint8_t* staging, const PatchWork& wk) {
   const int lane = threadIdx.x & 31;
@@ -405,7 +399,7 @@ __device__ __forceinline__ void tc_conv_patch_consumer(const TcConvParams& p, co
       mbar_arrive(&ctl->empty[prev]);
       if (prev_patch >= 0) mbar_arrive(&pc->pempty[prev_patch]);
     }
-    tc_conv_epilogue<NT>(p, pm, ctl, staging, acc, x0, y0, 0, 0, wk.n_off, stat_s1, stat_s2, p.bw == 16);
+    tc_conv_epilogue<NT>(p, ctl, staging, acc, x0, y0, 0, 0, wk.n_off, stat_s1, stat_s2, p.bw == 16);
   }
   tc_conv_stats_flush(p, wk.n_off, stat_s1, stat_s2);
 }
@@ -488,12 +482,12 @@ __device__ __forceinline__ void tc_conv_patch_body(const TcConvParams& p, uint8_
   } else if (warp >= 4) {
     // ===================================================================== wgmma + epilogue (one warpgroup)
     switch (nt) {
-      case 32: tc_conv_patch_consumer<BF16, 32>(p, &p, ctl, pc, patch_base, b_base, b_stage_bytes, staging, wk); break;
-      case 64: tc_conv_patch_consumer<BF16, 64>(p, &p, ctl, pc, patch_base, b_base, b_stage_bytes, staging, wk); break;
-      case 96: tc_conv_patch_consumer<BF16, 96>(p, &p, ctl, pc, patch_base, b_base, b_stage_bytes, staging, wk); break;
-      case 128: tc_conv_patch_consumer<BF16, 128>(p, &p, ctl, pc, patch_base, b_base, b_stage_bytes, staging, wk); break;
-      case 144: tc_conv_patch_consumer<BF16, 144>(p, &p, ctl, pc, patch_base, b_base, b_stage_bytes, staging, wk); break;
-      default: tc_conv_patch_consumer<BF16, 160>(p, &p, ctl, pc, patch_base, b_base, b_stage_bytes, staging, wk); break;
+      case 32: tc_conv_patch_consumer<BF16, 32>(p, ctl, pc, patch_base, b_base, b_stage_bytes, staging, wk); break;
+      case 64: tc_conv_patch_consumer<BF16, 64>(p, ctl, pc, patch_base, b_base, b_stage_bytes, staging, wk); break;
+      case 96: tc_conv_patch_consumer<BF16, 96>(p, ctl, pc, patch_base, b_base, b_stage_bytes, staging, wk); break;
+      case 128: tc_conv_patch_consumer<BF16, 128>(p, ctl, pc, patch_base, b_base, b_stage_bytes, staging, wk); break;
+      case 144: tc_conv_patch_consumer<BF16, 144>(p, ctl, pc, patch_base, b_base, b_stage_bytes, staging, wk); break;
+      default: tc_conv_patch_consumer<BF16, 160>(p, ctl, pc, patch_base, b_base, b_stage_bytes, staging, wk); break;
     }
   }
   __syncthreads();
@@ -600,13 +594,12 @@ __device__ __forceinline__ void tc_wgrad_transposer(const TcWgradParams& p, Smem
 
 // Warps 4-7 (one warpgroup): register-A wgmmas on the dY stage and the Bt tile, fp32 accumulators [2 m64 halves][NT / 2].
 // The A fragments of block n+1 are loaded while the wgmmas of block n run (two register sets, fa / fb), except at NT = 160,
-// where NT accumulators + 64 fragment registers do not fit in 255 registers, and inside the persistent deep-level kernel
-// (deep.cu), whose other ops already hold registers: there the loads wait for the wgmmas.
-template <int NT, bool DOUBLE>
+// where NT accumulators + 64 fragment registers do not fit in 255 registers: there the loads wait for the wgmmas.
+template <int NT>
 __device__ __forceinline__ void tc_wgrad_mma(const TcWgradParams& p, SmemCtlW* ctl, uint32_t stage_base, int stage_bytes,
                                              uint32_t bt_base, int items) {
   constexpr int kBt = wgrad_tbuf_bytes(false, NT);
-  constexpr bool kDouble = DOUBLE && NT <= 136;
+  constexpr bool kDouble = NT <= 136;
   const int et = threadIdx.x - 128;
   const int w = et >> 5, lane = et & 31, g = lane >> 2, t = lane & 3;
   const int taps = p.kh * p.kw;
@@ -779,19 +772,19 @@ __device__ __forceinline__ void tc_wgrad_consumer_bf16(const TcWgradParams& p, S
   }
 }
 
-template <bool DEEP, bool BF16, int NT>
+template <bool BF16, int NT>
 __device__ __forceinline__ void tc_wgrad_role(const TcWgradParams& p, SmemCtlW* ctl, uint8_t* smem, int stage_bytes,
                                               uint8_t* tbase, int items, int warp) {
   if constexpr (BF16) {
     if (warp >= 4) tc_wgrad_consumer_bf16<NT>(p, ctl, smem, stage_bytes, tbase, items);
   } else {
-    if (warp >= 4) tc_wgrad_mma<NT, !DEEP>(p, ctl, smem_u32(smem), stage_bytes, smem_u32(tbase), items);
+    if (warp >= 4) tc_wgrad_mma<NT>(p, ctl, smem_u32(smem), stage_bytes, smem_u32(tbase), items);
     else tc_wgrad_transposer<NT>(p, ctl, smem_u32(smem), stage_bytes, smem_u32(tbase), items);
   }
 }
 
-template <bool DEEP, bool BF16 = false>
-__device__ __forceinline__ void tc_wgrad_body(const TcWgradParams& p, const TcWgradParams* pm, uint8_t* smem_raw) {
+template <bool BF16>
+__device__ __forceinline__ void tc_wgrad_body(const TcWgradParams& p, uint8_t* smem_raw) {
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr int KE = BF16 ? 64 : 32;                           // channels per 128-byte row
   constexpr int YCH = 128 / KE;                                // chunks of dY (128 channels)
@@ -805,10 +798,10 @@ __device__ __forceinline__ void tc_wgrad_body(const TcWgradParams& p, const TcWg
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  if (!DEEP) pdl_trigger();
+  pdl_trigger();
   if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&pm->tmY);
-    tma_prefetch_desc(&pm->tmX);
+    tma_prefetch_desc(&p.tmY);
+    tma_prefetch_desc(&p.tmX);
   }
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < p.stages; ++i) {
@@ -821,7 +814,7 @@ __device__ __forceinline__ void tc_wgrad_body(const TcWgradParams& p, const TcWg
     }
     fence_mbar_init();
   }
-  if (!DEEP) pdl_wait();
+  pdl_wait();
   __syncthreads();
 
   if (warp == 0) {
@@ -846,9 +839,9 @@ __device__ __forceinline__ void tc_wgrad_body(const TcWgradParams& p, const TcWg
         uint8_t* sy = smem + stage * stage_bytes;
         if (elect_one()) {
           mbar_expect_tx(&ctl->full[stage], stage_bytes);
-          for (int j = 0; j < YCH; ++j) tma_load_3d(sy + j * chunk_bytes, &pm->tmY, &ctl->full[stage], j * KE, x0, y);
+          for (int j = 0; j < YCH; ++j) tma_load_3d(sy + j * chunk_bytes, &p.tmY, &ctl->full[stage], j * KE, x0, y);
           for (int j = 0; j < p.c_chunks; ++j)
-            tma_load_5d(sy + y_bytes + j * chunk_bytes, &pm->tmX, &ctl->full[stage], j * KE, cpx, cx, cpy, cy);
+            tma_load_5d(sy + y_bytes + j * chunk_bytes, &p.tmX, &ctl->full[stage], j * KE, cpx, cx, cpy, cy);
         }
         __syncwarp();
         if (++stage == p.stages) { stage = 0; phase ^= 1; }
@@ -856,23 +849,23 @@ __device__ __forceinline__ void tc_wgrad_body(const TcWgradParams& p, const TcWg
     }
   } else {
     switch (p.n_cols) {
-      case 32: tc_wgrad_role<DEEP, BF16, 32>(p, ctl, smem, stage_bytes, tbase, items, warp); break;
-      case 64: tc_wgrad_role<DEEP, BF16, 64>(p, ctl, smem, stage_bytes, tbase, items, warp); break;
-      case 96: tc_wgrad_role<DEEP, BF16, 96>(p, ctl, smem, stage_bytes, tbase, items, warp); break;
-      case 128: tc_wgrad_role<DEEP, BF16, 128>(p, ctl, smem, stage_bytes, tbase, items, warp); break;
-      case 136: tc_wgrad_role<DEEP, BF16, 136>(p, ctl, smem, stage_bytes, tbase, items, warp); break;
-      default: tc_wgrad_role<DEEP, BF16, 160>(p, ctl, smem, stage_bytes, tbase, items, warp); break;
+      case 32: tc_wgrad_role<BF16, 32>(p, ctl, smem, stage_bytes, tbase, items, warp); break;
+      case 64: tc_wgrad_role<BF16, 64>(p, ctl, smem, stage_bytes, tbase, items, warp); break;
+      case 96: tc_wgrad_role<BF16, 96>(p, ctl, smem, stage_bytes, tbase, items, warp); break;
+      case 128: tc_wgrad_role<BF16, 128>(p, ctl, smem, stage_bytes, tbase, items, warp); break;
+      case 136: tc_wgrad_role<BF16, 136>(p, ctl, smem, stage_bytes, tbase, items, warp); break;
+      default: tc_wgrad_role<BF16, 160>(p, ctl, smem, stage_bytes, tbase, items, warp); break;
     }
   }
   __syncthreads();
 }
 __global__ void __launch_bounds__(kNumThreads, 1) tc_wgrad_kernel(const __grid_constant__ TcWgradParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  tc_wgrad_body<false>(p, &p, smem_raw);
+  tc_wgrad_body<false>(p, smem_raw);
 }
 __global__ void __launch_bounds__(kNumThreads, 1) tc_wgrad_kernel_bf16(const __grid_constant__ TcWgradParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  tc_wgrad_body<false, true>(p, &p, smem_raw);
+  tc_wgrad_body<true>(p, smem_raw);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -925,12 +918,6 @@ cudaError_t tc_conv_launch(const TcConvParams& p, int num_sms, cudaStream_t s) {
   if (p.patch)
     return launch_k(p.bf16 ? tc_conv_patch_kernel_bf16 : tc_conv_patch_kernel, dim3(grid), dim3(kNumThreads), smem, s, 1, p);
   return launch_k(p.bf16 ? tc_conv_kernel_bf16 : tc_conv_kernel, dim3(grid), dim3(kNumThreads), smem, s, 1, p);
-}
-// grid the stand-alone launch uses (the persistent deep-level kernel runs the same CTA -> tile mapping on its first vgrid CTAs)
-int tc_conv_grid(const TcConvParams& p, int num_sms) {
-  const int tiles = p.tiles_x * p.tiles_y * (p.nphase > 0 ? p.nphase : 1);
-  if (p.n_split > 1) return tiles * p.n_split;
-  return tiles < num_sms ? tiles : num_sms;
 }
 
 cudaError_t tc_wgrad_launch(const TcWgradParams& p, cudaStream_t s) {

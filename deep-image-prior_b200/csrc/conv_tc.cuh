@@ -33,7 +33,6 @@ struct TcConvParams {
   // correlation over dY.  Work item = (phase, tile of the (h+1) x (w+1) phase grid); tmD is then the 5-D parity view
   // (C, px, X, py, Y) of the padded gradient buffer and the tile is stored at parity (opx, opy).  nphase = 0: one phase
   // described by kh / kw / offx / offy above, 3-D tmD.
-  int vgrid;               // deep-level kernel only: number of CTAs that work on this conv (= grid of the stand-alone launch)
   int nphase;
   struct Phase { int kh, kw, offx, offy, tap0, opx, opy; } phs[4];   // tap0: first packed weight tap of the phase
   int n_valid;             // output channels that exist (bias / statistics are only read / written below it); 0: all n_mma * n_split
@@ -78,7 +77,6 @@ size_t tc_conv_smem_bytes(const TcConvParams& p);
 size_t tc_wgrad_smem_bytes(const TcWgradParams& p);
 cudaError_t tc_conv_launch(const TcConvParams& p, int num_sms, cudaStream_t s);
 cudaError_t tc_wgrad_launch(const TcWgradParams& p, cudaStream_t s);
-int tc_conv_grid(const TcConvParams& p, int num_sms);
 cudaError_t tc_kernels_init();
 
 }  // namespace dip

@@ -16,7 +16,6 @@
 
 #include "../../include/dip.h"
 #include "conv_tc.cuh"
-#include "deep.cuh"
 #include "kernels.cuh"
 
 namespace dip {
@@ -62,7 +61,6 @@ static int engine_init() {
   g_encode = reinterpret_cast<PFN_encodeTiled>(fn);
   DIP_CUDA(tc_kernels_init());
   DIP_CUDA(down_kernels_init());
-  DIP_CUDA(deep_kernels_init());
   g_inited_mask |= 1ull << dev;
   return 0;
 }
@@ -176,15 +174,13 @@ enum HbmId { H_INPUT_PAD = 0, H_NOISE, H_SKINNY_FWD, H_BN_ACT_WRITE, H_BN_ACT_HE
 // ------------------------------------------------------------------------------------------------ conv op
 // CTAs per pixel tile (output channels split across them) for launches with fewer tiles than SMs: n_rows % (32 * split) == 0
 static int pick_nsplit(int tiles, int n_rows) {
-  int mx = 4;
-  if (const char* e = getenv("DIP_NSPLIT_MAX")) mx = atoi(e);
   int sp = 1;
-  while (sp * 2 <= mx && tiles * sp * 2 <= g_num_sms && n_rows % (32 * sp * 2) == 0) sp *= 2;
+  while (sp * 2 <= 4 && tiles * sp * 2 <= g_num_sms && n_rows % (32 * sp * 2) == 0) sp *= 2;
   return sp;
 }
-static void fit_stages(TcConvParams& p, size_t budget = 232448) {
+static void fit_stages(TcConvParams& p) {
   p.stages = p.patch ? 8 : 6;
-  while (tc_conv_smem_bytes(p) > budget && p.stages > 2) p.stages--;
+  while (tc_conv_smem_bytes(p) > 232448 && p.stages > 2) p.stages--;
 }
 struct ConvOp {
   Timer* timer = nullptr;
@@ -225,8 +221,7 @@ struct ConvOp {
   const float* wg_dy = nullptr; int wg_h = 0, wg_w = 0;
   // param slots
   int p_w = -1, p_b = -1;
-  TcConvParams fp{}, dg{};   // the general path (also the persistent deep-level kernel's ops)
-  TcConvParams fp_run{}, dg_run{};   // what the stand-alone launches run: fp / dg, or their stride-1 3x3 patch form
+  TcConvParams fp{}, dg{};   // what the launches run: the general form, or its stride-1 3x3 patch form
   TcWgradParams wg{};
   int simt_ksplits = 1;
 
@@ -257,20 +252,19 @@ struct ConvOp {
     return is_tc(prec) ? wacc_elems() : (size_t)simt_ksplits * k * k * 128 * c_pad;
   }
 
-  // The patch form q of a stride-1 3x3 conv g of the general path (tc_conv_patch_kernel): the same tiles, weights, output
-  // and N split, the activation [rows][cols][ld] (kc K channels) through the 4-D patch map.  It applies when the tile is 8
-  // or 16 pixels wide, the K channels fill whole 16-byte groups (TMA zero-fills the patch past the channel extent only in
-  // whole groups) and one patch per K block fits in shared memory beside at least two weight stages; otherwise q = g.  Both
-  // forms compute the same sums in the same order.  The persistent deep-level kernel always runs the general form.
-  int patch_form(const TcConvParams& g, TcConvParams& q, const void* act, int rows, int cols, int ld, int kc) {
-    q = g;
+  // Replaces the general form g of a stride-1 3x3 conv by its patch form (tc_conv_patch_kernel): the same tiles, weights,
+  // output and N split, the activation [rows][cols][ld] (kc K channels) through the 4-D patch map.  It applies when the tile
+  // is 8 or 16 pixels wide, the K channels fill whole 16-byte groups (TMA zero-fills the patch past the channel extent only
+  // in whole groups) and one patch per K block fits in shared memory beside at least two weight stages; otherwise g stays
+  // as it is.  Both forms compute the same sums in the same order.
+  int patch_form(TcConvParams& g, const void* act, int rows, int cols, int ld, int kc) {
     if ((g.bw != 8 && g.bw != 16) || kc % (bf16 ? 8 : 4) != 0 || g.kblocks > kPatchMaxKb) return 0;
     TcConvParams t = g;
     t.patch = 1;
     fit_stages(t);
     if (tc_conv_smem_bytes(t) > 232448) return 0;
     DIP_CHECK(map_patch(&t.tmA, act, rows, cols, ld, kc, g.bw, g.bh, bf16));
-    q = t;
+    g = t;
     return 0;
   }
   int build_tc(float* partial) {
@@ -294,9 +288,8 @@ struct ConvOp {
     fp.bias = nullptr; fp.stats = stats; fp.stats_ld = N;
     fit_stages(fp);
     }
-    fp_run = fp;
     if (do_fprop && k == 3 && stride == 1)
-      DIP_CHECK(bf16 ? patch_form(fp, fp_run, in16, in_rows, in_cols, in_ld16, C) : patch_form(fp, fp_run, in, in_rows, in_cols, in_ld, C));
+      DIP_CHECK(bf16 ? patch_form(fp, in16, in_rows, in_cols, in_ld16, C) : patch_form(fp, in, in_rows, in_cols, in_ld, C));
     // ---- dgrad
     if (has_dgrad && dg_s2) {
       // phase grid: (dg_out_h / 2) x (dg_out_w / 2) positions per parity class of the padded gradient
@@ -341,9 +334,8 @@ struct ConvOp {
       dg.bias = nullptr; dg.stats = nullptr; dg.stats_ld = 0;
       fit_stages(dg);
     }
-    dg_run = dg;
     if (has_dgrad && !dg_s2 && k == 3)
-      DIP_CHECK(bf16 ? patch_form(dg, dg_run, dg_in16, dg_in_h, dg_in_w, N, N) : patch_form(dg, dg_run, dg_in, dg_in_h, dg_in_w, N, N));
+      DIP_CHECK(bf16 ? patch_form(dg, dg_in16, dg_in_h, dg_in_w, N, N) : patch_form(dg, dg_in, dg_in_h, dg_in_w, N, N));
     // ---- wgrad
     wg = TcWgradParams{};
     if (!do_wgrad) return 0;
@@ -370,7 +362,7 @@ struct ConvOp {
 
   int run_fprop(int prec, const float* bias, cudaStream_t s) {
     if (is_tc(prec)) {
-      TcConvParams p = fp_run;
+      TcConvParams p = fp;
       p.bias = bias;
       TimeScope ts(timer, 0, alg_flops(), s);
       DIP_CUDA(tc_conv_launch(p, g_num_sms, s));
@@ -389,7 +381,7 @@ struct ConvOp {
   int run_dgrad(int prec, cudaStream_t s) {
     if (is_tc(prec)) {
       TimeScope ts(timer, 1, alg_flops(), s);
-      DIP_CUDA(tc_conv_launch(dg_run, g_num_sms, s));
+      DIP_CUDA(tc_conv_launch(dg, g_num_sms, s));
     } else {
       SimtConvArgs a{};
       a.A = dg_in; a.a_h = dg_in_h; a.a_w = dg_in_w; a.a_ld = N; a.a_c = N;
@@ -648,11 +640,6 @@ struct dip_plan {
   PackEntry* d_pack = nullptr; CvtEntry* d_cvt = nullptr; RunEntry* d_run = nullptr; UnpackEntry* d_unpack = nullptr;
   int n_pack = 0, n_cvt = 0, n_run = 0, n_unpack = 0;
   float* wacc_base = nullptr; size_t wacc_bytes = 0;   // all weight-gradient accumulators, contiguous
-  // persistent deep-level kernel (deep.cu): levels >= deep_from run as one launch per pass
-  static constexpr int kDeepMaxOps = 96;
-  DeepOp* d_deep_fwd = nullptr; DeepOp* d_deep_bwd = nullptr;
-  int n_deep_fwd = 0, n_deep_bwd = 0, deep_grid = 0, deep_from = 2;
-  unsigned* deep_bar = nullptr;
   long long pack_max = 0;
   bool bound = false;
   int nbt_is_float = 0;
@@ -923,7 +910,7 @@ static int build_plan(dip_plan* P, Arena& A) {
     a.out = v.raw_d1; a.out_h = v.h; a.out_w = v.w; a.stats = v.bn_d1.fwd;
     a.has_dgrad = l > 0 || d.input_grad != 0;
     a.dg_ld = v.Cin;   // level 0: stored depth (>= the conv's real input depth)
-    a.dg_s2 = bf || (prec == DIP_PRECISION_TF32 && getenv("DIP_ZERO_STUFF") == nullptr);   // A/B switch: the old zero-stuffed stride-1 dgrad
+    a.dg_s2 = is_tc(prec);   // (fp32 mode and 'avg' take the zero-stuffed stride-1 dgrad)
     if (a.dg_s2) { a.dg_in = v.dRaw_d1; a.dg_in_h = v.h; a.dg_in_w = v.w; }
     else { a.dg_in = v.ZS; a.dg_in_h = v.H; a.dg_in_w = v.W; }
     a.dg_out = v.dPin; a.dg_out_h = v.H + 2; a.dg_out_w = v.W + 2; a.dg_off = -2;
@@ -1010,11 +997,6 @@ static int build_plan(dip_plan* P, Arena& A) {
     for (ConvOp* op : P->convs) if (op->do_wgrad) { op->wacc = P->wacc_base ? P->wacc_base + off : nullptr; off += (op->wacc_elems() + 63) & ~size_t(63); }
   }
   P->d_unpack = A.get<UnpackEntry>(P->n_unpack > 0 ? P->n_unpack : 1);
-  P->d_deep_fwd = A.get<DeepOp>(dip_plan::kDeepMaxOps);
-  P->d_deep_bwd = A.get<DeepOp>(2 * dip_plan::kDeepMaxOps);
-  P->deep_bar = A.get<unsigned>(64);
-  if (const char* e = getenv("DIP_DEEP_FROM")) P->deep_from = atoi(e);
-  if (P->deep_from < 1) P->deep_from = 1;
   P->n_pack = (int)P->convs.size();
   P->n_cvt = (int)P->bns.size() * 3 + L + 2;
   P->n_run = (int)P->bns.size();
@@ -1145,16 +1127,6 @@ static const float* level_usrc(const dip_plan* P, int l) {
   return l == L - 1 ? P->lv[l].P_d2 : P->lv[l + 1].U;
 }
 
-// The persistent deep-level kernel (deep.cu) replaces the launches of levels >= deep_from (tensor-core precision, no
-// per-launch timers).  OPT-IN (DIP_DEEP=1): parity-green (tests/test_engine_gpu.py::test_deep_kernel_matches_launches) but
-// not the default: the small kernels are bounded by their own prologue + a few memory round trips rather than by launch
-// gaps, and one 256-thread CTA per SM (the conv code lives in the same kernel) has far fewer loads in flight than the
-// stand-alone kernels.  Its speed on H100 has not been measured.
-static bool deep_on(const dip_plan* P) {
-  const char* e = getenv("DIP_DEEP");   // read per call: the test switches it inside one process
-  return e != nullptr && e[0] == '1' && P->desc.precision == DIP_PRECISION_TF32 && !P->timer.on && P->n_deep_fwd > 0 &&
-         (int)P->lv.size() > P->deep_from;
-}
 static int fwd_level(dip_plan* P, int l, cudaStream_t s, int& nl) {
   Level& v = P->lv[l];
   const int prec = P->desc.precision;
@@ -1192,15 +1164,7 @@ static int fwd_level(dip_plan* P, int l, cudaStream_t s, int& nl) {
         launch_bn_act_write(v.raw_d2, nd, bn_ref(P, v.bn_d2), v.h, v.w, (bf && !last && P->lv[l + 1].ns != 4) ? nullptr : v.P_d2, nd, last ? 0 : 1, 1, s,
                             Twin{last ? nullptr : v.P_d2_16, nd}, P->zero_pad));   // (the 4-channel skip conv of the next level reads the fp32 tensor)
   nl += 4 + (prec == DIP_PRECISION_FP32 ? 2 : 0);
-  if (!last) {
-    if (deep_on(P) && l + 1 == P->deep_from) {
-      // every level below this one: ONE persistent launch (deep.cu) instead of ~13 launches per level
-      DIP_CUDA(launch_deep(P->d_deep_fwd, P->n_deep_fwd, P->deep_bar, P->deep_grid, s));
-      nl += 2;
-    } else {
-      DIP_CHECK(fwd_level(P, l + 1, s, nl));
-    }
-  }
+  if (!last) DIP_CHECK(fwd_level(P, l + 1, s, nl));
   // upsample + concat + BN + pad
   if (CS > 0) join_skip(P, s);
   CatArgs ca = cat_args(P, v, level_usrc(P, l));
@@ -1300,16 +1264,9 @@ static GradSrc src_fold(const float* gp, int ld, const float* ds, const float* w
 }
 static GradSrc src_upadj(const float* d, int ld, int bilinear) { GradSrc s{}; s.kind = 2; s.g = d; s.ld = ld; s.coff = 0; s.bilinear = bilinear; return s; }
 
-// Weight gradient (side stream) and input gradient (main stream, on the critical path) of one conv.  Both are persistent
-// kernels that fill every SM, so they run one after the other whichever way: the dgrad is enqueued first and the main
-// stream has the higher priority, so that the wgrad overlaps the HBM-bound kernels that follow the dgrad instead of
-// delaying it.  (DIP_WGRAD_FIRST=1: the old order, for A/B runs.)
-static int defer_level() {
-  // weight gradients of the levels above this index are deferred until the backward pass reaches it, so that they run
-  // beside the deeper levels' launches
-  static const int lv = getenv("DIP_DEFER_WGRAD") ? atoi(getenv("DIP_DEFER_WGRAD")) : 2;   // 0: no deferral
-  return lv;
-}
+// Weight gradients of the levels above kDeferLevel are deferred until the backward pass reaches it, so that they run
+// beside the deeper levels' launches.
+static constexpr int kDeferLevel = 2;
 static int flush_deferred(dip_plan* P, int prec, cudaStream_t s) {
   if (P->deferred.empty()) return 0;
   cudaStream_t ws = fork_side(P, s);
@@ -1317,25 +1274,19 @@ static int flush_deferred(dip_plan* P, int prec, cudaStream_t s) {
   P->deferred.clear();
   return 0;
 }
+// Weight gradient (side stream) and input gradient (main stream, on the critical path) of one conv.  Both are persistent
+// kernels that fill every SM, so they run one after the other whichever way: the dgrad is enqueued first and the main
+// stream has the higher priority, so that the wgrad overlaps the HBM-bound kernels that follow the dgrad instead of
+// delaying it.
 static int conv_backward(dip_plan* P, ConvOp& op, bool dgrad, int prec, cudaStream_t s, int level = 99) {
-  static const bool wgrad_first = getenv("DIP_WGRAD_FIRST") != nullptr;
-  if (P->side_on && level < defer_level() && (int)P->lv.size() > defer_level()) {
+  if (P->side_on && level < kDeferLevel && (int)P->lv.size() > kDeferLevel) {
     if (dgrad) DIP_CHECK(op.run_dgrad(prec, s));
     P->deferred.push_back(&op);
     return 0;
   }
-  static const bool after_dgrad = getenv("DIP_WGRAD_AFTER_DGRAD") != nullptr;
-  if (after_dgrad) {
-    // the wgrad becomes runnable only once its sibling dgrad has finished: it then starts beside the HBM-bound kernels
-    // that follow the dgrad instead of fighting it for the SMs
-    if (dgrad) DIP_CHECK(op.run_dgrad(prec, s));
-    return op.run_wgrad(prec, P->partial, P->grads[op.p_w], fork_side(P, s));
-  }
   cudaStream_t ws = fork_side(P, s);
-  if (wgrad_first) DIP_CHECK(op.run_wgrad(prec, P->partial, P->grads[op.p_w], ws));
   if (dgrad) DIP_CHECK(op.run_dgrad(prec, s));
-  if (!wgrad_first) DIP_CHECK(op.run_wgrad(prec, P->partial, P->grads[op.p_w], ws));
-  return 0;
+  return op.run_wgrad(prec, P->partial, P->grads[op.p_w], ws);
 }
 
 static int bwd_level(dip_plan* P, int l, GradSrc src_v, cudaStream_t s, int& nl) {
@@ -1347,7 +1298,7 @@ static int bwd_level(dip_plan* P, int l, GradSrc src_v, cudaStream_t s, int& nl)
   const int wl = is_tc(prec) ? 1 : 2;   // tensor-core wgrads accumulate in place (no per-conv reduction launch)
   // 1x1 conv + BN + LReLU
   DIP_CHECK(bn_bwd(P, v.raw_v, nu, v.bn_v, 1, src_v, v.H, v.W, v.dRaw_v, nullptr, s, nl, v.dRaw_v16));
-  if (l == defer_level()) DIP_CHECK(flush_deferred(P, prec, s));
+  if (l == kDeferLevel) DIP_CHECK(flush_deferred(P, prec, s));
   DIP_CHECK(conv_backward(P, v.c11, true, prec, s, l));
   nl += wl + 1;
   // up conv + BN + LReLU
@@ -1394,13 +1345,7 @@ static int bwd_level(dip_plan* P, int l, GradSrc src_v, cudaStream_t s, int& nl)
   // deeper branch
   GradSrc src_d2;
   if (!last) {
-    if (deep_on(P) && P->n_deep_bwd > 0 && l + 1 == P->deep_from) {
-      if (P->deep_from >= defer_level()) DIP_CHECK(flush_deferred(P, prec, s));   // outer-level wgrads run beside the deep kernel
-      DIP_CUDA(launch_deep(P->d_deep_bwd, P->n_deep_bwd, P->deep_bar + 16, P->deep_grid, s));
-      nl += 2;
-    } else {
-      DIP_CHECK(bwd_level(P, l + 1, src_plain(v.dUp, v.cu, 0), s, nl));
-    }
+    DIP_CHECK(bwd_level(P, l + 1, src_plain(v.dUp, v.cu, 0), s, nl));
     join_skip(P, s);   // the next level's skip-branch gradients (dRaw_s / dS) feed the BN backward below
     Level& n = P->lv[l + 1];   // (its input depth n.Cin == nd)
     if (n.ns == 128) { src_d2 = src_fold(n.dPin, nd, nullptr, nullptr, 0); src_d2.add = n.dS; src_d2.ld_add = nd; }
@@ -1423,173 +1368,6 @@ static int bwd_level(dip_plan* P, int l, GradSrc src_v, cudaStream_t s, int& nl)
   DIP_CHECK(conv_backward(P, v.d1, d1_dgrad, prec, s));
   nl += wl + (d1_dgrad ? 1 : 0);
   DIP_CUDA(cudaGetLastError());
-  return 0;
-}
-
-// ------------------------------------------------------------------------------------------------ deep-level op lists
-static void vec_lanes(int C, int* VL, int* PPB) { *VL = C / 4; *PPB = 256 / *VL; if (*PPB < 1) *PPB = 1; }
-static DeepOp deep_conv(dip_plan* P, const TcConvParams& src, const float* bias, double* stats, int sync = 1) {
-  DeepOp o;
-  o.type = DO_CONV; o.sync = sync;
-  o.u.conv = src;
-  o.u.conv.bias = bias;
-  o.u.conv.stats = stats;
-  fit_stages(o.u.conv, deep_dyn_smem());
-  o.u.conv.vgrid = tc_conv_grid(o.u.conv, g_num_sms);
-  if (o.u.conv.vgrid > P->deep_grid) P->deep_grid = o.u.conv.vgrid;
-  return o;
-}
-static DeepOp deep_bn_act_write(dip_plan* P, const float* raw, const BnLayer& b, int H, int W, float* dst, int pad) {
-  DeepOp o;
-  o.type = DO_BN_ACT_WRITE;
-  vec_lanes(b.C, &o.VL, &o.PPB);
-  o.u.bnw = DeepBnActWrite{raw, b.C, bn_ref(P, b), H, W, dst, b.C, pad, 1};
-  return o;
-}
-static void deep_fwd_level(dip_plan* P, int l, std::vector<DeepOp>& ops) {
-  Level& v = P->lv[l];
-  const int CS = v.ns;
-  const bool last = l == (int)P->lv.size() - 1;
-  const float* pin_interior = v.Pin + ((size_t)(v.W + 2) + 1) * v.Cin;
-  // skip branch (independent of the deeper branch until the concat: no barrier behind it)
-  if (CS == 128) {
-    ops.push_back(deep_conv(P, v.sk.fp, P->params[v.p_skip_b], v.bn_s.fwd, 0));
-  } else {
-    DeepOp o;
-    o.type = DO_SKINNY_FWD; o.sync = 0;
-    o.u.skf = DeepSkinnyFwd{pin_interior, v.Cin, v.W + 2, P->params[v.p_skip_w], P->params[v.p_skip_b], v.Cin, CS, v.H, v.W, v.raw_s,
-                            0, v.bn_s.fwd, v.Cin_act};
-    ops.push_back(o);
-  }
-  ops.push_back(deep_conv(P, v.d1.fp, P->params[v.d1.p_b], v.bn_d1.fwd));
-  ops.push_back(deep_bn_act_write(P, v.raw_d1, v.bn_d1, v.h, v.w, v.P_d1, 1));
-  ops.push_back(deep_conv(P, v.d2.fp, P->params[v.d2.p_b], v.bn_d2.fwd));
-  ops.push_back(deep_bn_act_write(P, v.raw_d2, v.bn_d2, v.h, v.w, v.P_d2, last ? 0 : 1));
-  if (!last) deep_fwd_level(P, l + 1, ops);
-  {
-    DeepOp o;
-    o.type = DO_CAT_STATS;
-    vec_lanes(v.cu + CS, &o.VL, &o.PPB);
-    o.u.cat = DeepCat{cat_args(P, v, level_usrc(P, l)), v.bn_cat.fwd, bn_ref(P, v.bn_cat), v.P_cat};
-    ops.push_back(o);
-    o.type = DO_CAT_WRITE;
-    ops.push_back(o);
-  }
-  ops.push_back(deep_conv(P, v.up.fp, P->params[v.up.p_b], v.bn_u.fwd));
-  {
-    DeepOp o = deep_bn_act_write(P, v.raw_u, v.bn_u, v.H, v.W, v.A_u, 0);
-    ops.push_back(o);
-  }
-  ops.push_back(deep_conv(P, v.c11.fp, P->params[v.c11.p_b], v.bn_v.fwd));
-  ops.push_back(deep_bn_act_write(P, v.raw_v, v.bn_v, v.H, v.W, v.U, 0));
-}
-static void deep_bn_bwd(dip_plan* P, const float* raw, int ld_raw, BnLayer& b, GradSrc src, int H, int W, float* draw,
-                        std::vector<DeepOp>& ops, int sync_last = 1) {
-  DeepOp o;
-  o.type = DO_BN_BWD_REDUCE;
-  vec_lanes(b.C, &o.VL, &o.PPB);
-  o.u.bnb = DeepBnBwd{raw, ld_raw, bn_ref(P, b), 1, src, H, W, b.bwd, draw, nullptr, b.dbias};
-  ops.push_back(o);
-  o.type = DO_BN_BWD_APPLY; o.sync = sync_last;
-  ops.push_back(o);
-}
-static DeepOp deep_wgrad(dip_plan* P, const ConvOp& op, int sync = 1) {
-  DeepOp o;
-  o.type = DO_WGRAD; o.sync = sync;
-  o.u.wg = op.wg;
-  o.u.wg.partial = op.wacc;
-  while (tc_wgrad_smem_bytes(o.u.wg) > deep_dyn_smem() && o.u.wg.stages > 1) o.u.wg.stages--;
-  return o;
-}
-static void deep_bwd_level(dip_plan* P, int l, GradSrc src_v, std::vector<DeepOp>& ops) {
-  Level& v = P->lv[l];
-  const int CS = v.ns, CC = v.cu + v.ns;
-  const bool last = l == (int)P->lv.size() - 1;
-  // 1x1 conv + BN + LReLU
-  deep_bn_bwd(P, v.raw_v, 128, v.bn_v, src_v, v.H, v.W, v.dRaw_v, ops);
-  ops.push_back(deep_conv(P, v.c11.dg, nullptr, nullptr, 0));
-  ops.push_back(deep_wgrad(P, v.c11));
-  // up conv + BN + LReLU
-  deep_bn_bwd(P, v.raw_u, 128, v.bn_u, src_plain(v.dA_u, 128, 0), v.H, v.W, v.dRaw_u, ops);
-  if (CS == 128) {
-    ops.push_back(deep_conv(P, v.up_a.dg, nullptr, nullptr, 0));
-    ops.push_back(deep_conv(P, v.up_b.dg, nullptr, nullptr, 0));
-    ops.push_back(deep_wgrad(P, v.up_a, 0));
-    ops.push_back(deep_wgrad(P, v.up_b));
-  } else {
-    ops.push_back(deep_conv(P, v.up.dg, nullptr, nullptr, 0));
-    ops.push_back(deep_wgrad(P, v.up));
-  }
-  // concat BN
-  {
-    DeepOp o;
-    o.type = DO_CAT_BWD_REDUCE;
-    vec_lanes(CC, &o.VL, &o.PPB);
-    o.u.catb = DeepCatBwd{v.P_cat, bn_ref(P, v.bn_cat), v.dP_cat, CC, v.H, v.W, v.bn_cat.bwd, v.dCat};
-    ops.push_back(o);
-    o.type = DO_CAT_BWD_APPLY;
-    ops.push_back(o);
-  }
-  {
-    DeepOp o;   // adjoint of the x2 upsampling; the skip-branch ops behind it only read dCat as well: no barrier
-    o.type = DO_UPADJ; o.sync = 0;
-    vec_lanes(128, &o.VL, &o.PPB);
-    o.u.up = DeepUpadj{v.dCat, CC, 0, v.h, v.w, 128, v.bilinear, v.dUp};
-    ops.push_back(o);
-  }
-  // skip branch
-  deep_bn_bwd(P, v.raw_s, CS, v.bn_s, src_plain(v.dCat, CC, 128), v.H, v.W, v.dRaw_s, ops);
-  if (CS == 128) {
-    ops.push_back(deep_conv(P, v.sk.dg, nullptr, nullptr, 0));   // dS (levels > 0 always need it)
-    ops.push_back(deep_wgrad(P, v.sk));
-  } else {
-    const float* pin_interior = v.Pin + ((size_t)(v.W + 2) + 1) * v.Cin;
-    DeepOp o;
-    o.type = DO_SKINNY_BWD; o.sync = 1;
-    vec_lanes(v.Cin, &o.VL, &o.PPB);
-    o.u.skb = DeepSkinnyBwd{pin_interior, v.Cin, v.W + 2, P->params[v.p_skip_w], v.Cin, CS, v.H, v.W, v.dRaw_s, nullptr, 0, nullptr,
-                            v.dw_s, nullptr, v.Cin_act};
-    ops.push_back(o);
-  }
-  // deeper branch
-  GradSrc src_d2;
-  if (!last) {
-    deep_bwd_level(P, l + 1, src_plain(v.dUp, 128, 0), ops);
-    Level& n = P->lv[l + 1];
-    if (CS == 128) { src_d2 = src_fold(n.dPin, 128, nullptr, nullptr, 0); src_d2.add = n.dS; src_d2.ld_add = 128; }
-    else src_d2 = src_fold(n.dPin, 128, n.dRaw_s, P->params[n.p_skip_w], CS);
-  } else {
-    src_d2 = src_plain(v.dUp, 128, 0);
-  }
-  deep_bn_bwd(P, v.raw_d2, 128, v.bn_d2, src_d2, v.h, v.w, v.dRaw_d2, ops);
-  ops.push_back(deep_conv(P, v.d2.dg, nullptr, nullptr, 0));
-  ops.push_back(deep_wgrad(P, v.d2));
-  deep_bn_bwd(P, v.raw_d1, 128, v.bn_d1, src_fold(v.dP_d1, 128, nullptr, nullptr, 0), v.h, v.w, v.dRaw_d1, ops);
-  ops.push_back(deep_conv(P, v.d1.dg, nullptr, nullptr, 0));     // 4-phase stride-2 input gradient -> dPin
-  ops.push_back(deep_wgrad(P, v.d1));
-}
-static int build_deep_ops(dip_plan* P) {
-  P->n_deep_fwd = P->n_deep_bwd = 0;
-  P->deep_grid = 128 < g_num_sms ? 128 : g_num_sms;
-  // (the op lists write and fold reflection halos only: a zero-padded network keeps the launch-by-launch path)
-  if (P->desc.precision != DIP_PRECISION_TF32 || (int)P->lv.size() <= P->deep_from || P->zero_pad) return 0;
-  // the op lists below are written for the 128-wide stride-2 network with the same skip branch (4 or 128 channels) at
-  // every scale: they have no pooling pass (downsample_mode 'avg' normalises the pooled raw_d1, which only fwd_level writes)
-  for (const Level& v : P->lv)
-    if (v.nd != 128 || v.nu != 128 || v.ns == 0 || v.ns != P->lv[0].ns || v.rawF != nullptr) return 0;
-  std::vector<DeepOp> fwd;
-  deep_fwd_level(P, P->deep_from, fwd);
-  if ((int)fwd.size() > dip_plan::kDeepMaxOps) return fail("internal: deep forward op list too long");
-  DIP_CUDA(cudaMemcpy(P->d_deep_fwd, fwd.data(), fwd.size() * sizeof(DeepOp), cudaMemcpyHostToDevice));
-  P->n_deep_fwd = (int)fwd.size();
-  if (getenv("DIP_NO_DEEP_BWD") == nullptr && P->lv[P->deep_from].d1.dg_s2) {
-    std::vector<DeepOp> bwd;
-    deep_bwd_level(P, P->deep_from, src_plain(P->lv[P->deep_from - 1].dUp, 128, 0), bwd);
-    if ((int)bwd.size() > 2 * dip_plan::kDeepMaxOps) return fail("internal: deep backward op list too long");
-    DIP_CUDA(cudaMemcpy(P->d_deep_bwd, bwd.data(), bwd.size() * sizeof(DeepOp), cudaMemcpyHostToDevice));
-    P->n_deep_bwd = (int)bwd.size();
-  }
-  if (P->deep_grid > g_num_sms) P->deep_grid = g_num_sms;
   return 0;
 }
 
@@ -1754,7 +1532,6 @@ int dip_plan_bind(dip_plan* P, void* const* params, void* const* grads, void* co
   P->running.clear();
   if (bn_running != nullptr) P->running.assign(bn_running, bn_running + 3 * P->bns.size());
   DIP_CHECK(upload_tables(P));
-  DIP_CHECK(build_deep_ops(P));
   P->bound = true;
   return 0;
 }
@@ -1887,8 +1664,7 @@ static int run_body(dip_plan* P, dip_adam* adam, const float* z0, const float* t
     plan_pack(P, fork_side(P, s));
     P->prepacked = true;
   }
-  static const bool split_noise = getenv("DIP_SPLIT_NOISE") != nullptr;   // A/B switch: separate k_noise + k_input_pad launches
-  if (sigma > 0.f && (split_noise || P->W % 4 != 0)) {
+  if (sigma > 0.f && P->W % 4 != 0) {   // the fused k_noise_pad needs W % 4 == 0: separate k_noise + k_input_pad launches
     HBM_T(&P->timer, H_NOISE, 0, 2.0 * nz * sizeof(float), s, launch_noise(z0, P->zbuf, sigma, seed, (uint64_t)step_base, it_dev, nz, s));
     zin = P->zbuf;
   } else if (sigma > 0.f) {

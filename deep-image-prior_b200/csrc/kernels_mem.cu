@@ -172,7 +172,7 @@ __device__ __forceinline__ void block_reduce_atomic(float4 (&acc)[K], int VL, in
   } else {
     nparts = PPB;
     part = tid / VL;
-    if (part < nparts) {   // (a 256-thread block of the persistent deep-level kernel has idle threads when VL * PPB < 256)
+    if (part < nparts) {
 #pragma unroll
       for (int k = 0; k < K; ++k) red_smem[(k * nparts + part) * VL + (tid % VL)] = acc[k];
     }
@@ -323,10 +323,11 @@ void launch_channel_stats(const float* x, int ld, int C, int npix, double* fwd, 
 
 // ------------------------------------------------------------------------------------------------ bn_act_write
 // ZP: with pad, the halo cells are written as 0 (their load reads the nearest interior pixel, whose value is discarded)
-template <bool ZP = false>
-__device__ __forceinline__ void d_bn_act_write(const float* __restrict__ raw, int ld_in, BnRef bn, int H, int W,
+template <bool ZP>
+__global__ void __launch_bounds__(256) k_bn_act_write(const float* __restrict__ raw, int ld_in, BnRef bn, int H, int W,
                                                       float* __restrict__ dst, int ld_out, int pad, int act, int VL,
-                                                      int PPB, Twin t16 = kNoTwin) {
+                                                      int PPB, Twin t16) {
+  pdl_enter();
   const int v = threadIdx.x % VL, slot = threadIdx.x / VL;
   const Bn4 cf = bn_coef<0>(bn, v);
   const int Ho = H + 2 * pad, Wo = W + 2 * pad;
@@ -347,13 +348,6 @@ __device__ __forceinline__ void d_bn_act_write(const float* __restrict__ raw, in
                  if (dst != nullptr) st4(dst + static_cast<size_t>(p) * ld_out + 4 * v, y);
                  if (t16.p != nullptr) st4_bf16(t16.p + static_cast<size_t>(p) * t16.ld + 4 * v, y);
                });
-}
-template <bool ZP>
-__global__ void __launch_bounds__(256) k_bn_act_write(const float* __restrict__ raw, int ld_in, BnRef bn, int H, int W,
-                                                      float* __restrict__ dst, int ld_out, int pad, int act, int VL,
-                                                      int PPB, Twin t16) {
-  pdl_enter();
-  d_bn_act_write<ZP>(raw, ld_in, bn, H, W, dst, ld_out, pad, act, VL, PPB, t16);
 }
 void launch_bn_act_write(const float* raw, int ld_in, BnRef bn, int H, int W, float* dst, int ld_out, int pad,
                          int act, cudaStream_t s, Twin t16, int zero_pad) {
@@ -454,7 +448,8 @@ __device__ __forceinline__ void cat_quad(const CatArgs& a, const CatLane& l, int
   }
 }
 
-__device__ __forceinline__ void d_cat_stats(CatArgs a, double* __restrict__ fwd, int VL, int PPB) {
+__global__ void __launch_bounds__(256, DIP_CAT_MINBLOCKS) k_cat_stats(CatArgs a, double* __restrict__ fwd, int VL, int PPB) {
+  pdl_enter();
   const int v = threadIdx.x % VL, slot = threadIdx.x / VL;
   const CatLane l = cat_lane(a, v);
   const int w = a.W >> 1, nsrc = (a.H >> 1) * w;
@@ -472,10 +467,6 @@ __device__ __forceinline__ void d_cat_stats(CatArgs a, double* __restrict__ fwd,
   double* const dst[2] = {fwd, fwd + (a.Cu + a.Cs) * kAccS};
   const int wid[2] = {a.Cu + a.Cs, a.Cu + a.Cs};
   block_reduce_atomic<2>(acc, VL, PPB, dst, wid);
-}
-__global__ void __launch_bounds__(256, DIP_CAT_MINBLOCKS) k_cat_stats(CatArgs a, double* __restrict__ fwd, int VL, int PPB) {
-  pdl_enter();
-  d_cat_stats(a, fwd, VL, PPB);
 }
 void launch_cat_stats(CatArgs a, double* fwd_cat, cudaStream_t s) {
   VecGeom g = vec_geom(a.Cu + a.Cs, static_cast<long long>(a.H / 2) * (a.W / 2));
@@ -506,8 +497,9 @@ __device__ __forceinline__ void store_with_halo(float* __restrict__ dst, int ld,
     }
 }
 
-template <bool ZP = false>
-__device__ __forceinline__ void d_cat_write(CatArgs a, BnRef bn_cat, float* __restrict__ dst, int VL, int PPB, Twin t16 = kNoTwin) {
+template <bool ZP>
+__global__ void __launch_bounds__(256, DIP_CAT_MINBLOCKS) k_cat_write(CatArgs a, BnRef bn_cat, float* __restrict__ dst, int VL, int PPB, Twin t16) {
+  pdl_enter();
   const int v = threadIdx.x % VL, slot = threadIdx.x / VL;
   const CatLane l = cat_lane(a, v);
   const Bn4 cf = bn_coef<0>(bn_cat, v);
@@ -521,11 +513,6 @@ __device__ __forceinline__ void d_cat_write(CatArgs a, BnRef bn_cat, float* __re
     for (int e = 0; e < 4; ++e)
       store_with_halo<ZP>(dst, ld, a.H, a.W, 2 * si + (e >> 1), 2 * sj + (e & 1), v, bn_apply(cf, q[e]), t16);
   }
-}
-template <bool ZP>
-__global__ void __launch_bounds__(256, DIP_CAT_MINBLOCKS) k_cat_write(CatArgs a, BnRef bn_cat, float* __restrict__ dst, int VL, int PPB, Twin t16) {
-  pdl_enter();
-  d_cat_write<ZP>(a, bn_cat, dst, VL, PPB, t16);
 }
 void launch_cat_write(CatArgs a, BnRef bn_cat, float* dst, cudaStream_t s, Twin t16, int zero_pad) {
   VecGeom g = vec_geom(a.Cu + a.Cs, static_cast<long long>(a.H / 2) * (a.W / 2));
@@ -834,10 +821,10 @@ void launch_bn_bwd_reduce(const float* raw, int ld_raw, BnRef bn, int act, GradS
 // apply pass; for the head source (KIND 3) it also accumulates the head's own gradients:
 //   dW_head[k][c] += dl[k] * act(bn(raw))[c],  db_head[k] += dl[k]
 template <int KIND, bool ZP = false>
-__device__ __forceinline__ void d_bn_bwd_apply(const float* __restrict__ raw, int ld_raw, BnRef bn, int act, GradSrc src,
+__global__ void __launch_bounds__(256, KIND == 2 ? 3 : 2) k_bn_bwd_apply(const float* __restrict__ raw, int ld_raw, BnRef bn, int act, GradSrc src,
                                                       int H, int W, const double* __restrict__ bwd, float* __restrict__ draw,
-                                                      float* __restrict__ zs, double* __restrict__ dbias, int VL, int PPB,
-                                                      Twin t16 = kNoTwin) {
+                                                      float* __restrict__ zs, double* __restrict__ dbias, int VL, int PPB, Twin t16) {
+  pdl_enter();
   const int v = threadIdx.x % VL, slot = threadIdx.x / VL;
   const Bn4 cf = bn_coef<0>(bn, v);
   const SrcRegs sr = src_regs<KIND>(src, bn.C, v);
@@ -915,13 +902,6 @@ __device__ __forceinline__ void d_bn_bwd_apply(const float* __restrict__ raw, in
     block_reduce_atomic<K>(acc, VL, PPB, dst, wid);
   }
 }
-template <int KIND, bool ZP = false>
-__global__ void __launch_bounds__(256, KIND == 2 ? 3 : 2) k_bn_bwd_apply(const float* __restrict__ raw, int ld_raw, BnRef bn, int act, GradSrc src,
-                                                      int H, int W, const double* __restrict__ bwd, float* __restrict__ draw,
-                                                      float* __restrict__ zs, double* __restrict__ dbias, int VL, int PPB, Twin t16) {
-  pdl_enter();
-  d_bn_bwd_apply<KIND, ZP>(raw, ld_raw, bn, act, src, H, W, bwd, draw, zs, dbias, VL, PPB, t16);
-}
 void launch_bn_bwd_apply(const float* raw, int ld_raw, BnRef bn, int act, GradSrc src, int H, int W,
                          const double* bwd, float* draw, float* zs, double* dbias, cudaStream_t s, Twin t16) {
   VecGeom g = vec_geom(bn.C, static_cast<long long>(H) * W);
@@ -963,9 +943,10 @@ __device__ __forceinline__ float4 cat_xhat(const CatBwdCoef& c, float4 y) {
   return make_float4((y.x - c.beta.x) * c.inv_gamma.x, (y.y - c.beta.y) * c.inv_gamma.y, (y.z - c.beta.z) * c.inv_gamma.z,
                      (y.w - c.beta.w) * c.inv_gamma.w);
 }
-template <bool ZP = false>
-__device__ __forceinline__ void d_cat_bwd_reduce(const float* __restrict__ pcat, BnRef bn_cat, const float* __restrict__ gp,
+template <bool ZP>
+__global__ void __launch_bounds__(256) k_cat_bwd_reduce(const float* __restrict__ pcat, BnRef bn_cat, const float* __restrict__ gp,
                                                         int ld, int H, int W, double* __restrict__ bwd, int VL, int PPB) {
+  pdl_enter();
   const int v = threadIdx.x % VL, slot = threadIdx.x / VL;
   const CatBwdCoef cf = cat_bwd_coef(bn_cat, v);
   const int Wp = W + 2;
@@ -987,12 +968,6 @@ __device__ __forceinline__ void d_cat_bwd_reduce(const float* __restrict__ pcat,
   const int wid[2] = {bn_cat.C, bn_cat.C};
   block_reduce_atomic<2>(acc, VL, PPB, dst, wid);
 }
-template <bool ZP>
-__global__ void __launch_bounds__(256) k_cat_bwd_reduce(const float* __restrict__ pcat, BnRef bn_cat, const float* __restrict__ gp,
-                                                        int ld, int H, int W, double* __restrict__ bwd, int VL, int PPB) {
-  pdl_enter();
-  d_cat_bwd_reduce<ZP>(pcat, bn_cat, gp, ld, H, W, bwd, VL, PPB);
-}
 void launch_cat_bwd_reduce(const float* pcat, BnRef bn_cat, const float* gp, int ld, int H, int W, double* bwd,
                            cudaStream_t s, int zero_pad) {
   VecGeom g = vec_geom(bn_cat.C, static_cast<long long>(H) * W);
@@ -1000,10 +975,11 @@ void launch_cat_bwd_reduce(const float* pcat, BnRef bn_cat, const float* gp, int
   fit_grid(g, kernel, red_bytes(g, 2));
   launch_red(kernel, g.blocks, g.threads, red_bytes(g, 2), s, pcat, bn_cat, gp, ld, H, W, bwd, g.VL, g.PPB);
 }
-template <bool ZP = false>
-__device__ __forceinline__ void d_cat_bwd_apply(const float* __restrict__ pcat, BnRef bn_cat, const float* __restrict__ gp,
+template <bool ZP>
+__global__ void __launch_bounds__(256) k_cat_bwd_apply(const float* __restrict__ pcat, BnRef bn_cat, const float* __restrict__ gp,
                                                        int ld, int H, int W, const double* __restrict__ bwd,
                                                        float* __restrict__ dcat, int VL, int PPB) {
+  pdl_enter();
   const int v = threadIdx.x % VL, slot = threadIdx.x / VL;
   const CatBwdCoef cf = cat_bwd_coef(bn_cat, v);
   const int C = bn_cat.C;
@@ -1028,13 +1004,6 @@ __device__ __forceinline__ void d_cat_bwd_apply(const float* __restrict__ pcat, 
                  st4(dcat + static_cast<size_t>(p) * C + 4 * v, dx);
                });
 }
-template <bool ZP>
-__global__ void __launch_bounds__(256) k_cat_bwd_apply(const float* __restrict__ pcat, BnRef bn_cat, const float* __restrict__ gp,
-                                                       int ld, int H, int W, const double* __restrict__ bwd,
-                                                       float* __restrict__ dcat, int VL, int PPB) {
-  pdl_enter();
-  d_cat_bwd_apply<ZP>(pcat, bn_cat, gp, ld, H, W, bwd, dcat, VL, PPB);
-}
 void launch_cat_bwd_apply(const float* pcat, BnRef bn_cat, const float* gp, int ld, int H, int W, const double* bwd,
                           float* dcat, cudaStream_t s, int zero_pad) {
   VecGeom g = vec_geom(bn_cat.C, static_cast<long long>(H) * W);
@@ -1044,8 +1013,9 @@ void launch_cat_bwd_apply(const float* pcat, BnRef bn_cat, const float* gp, int 
 }
 
 // Adjoint of the x2 upsampling, materialised once: dst[h][w][C] <- D[2h][2w][ld] (channels coff..coff+C)
-__device__ __forceinline__ void d_upadj(const float* __restrict__ D, int ld, int coff, int h, int w, int C, int bilinear,
+__global__ void __launch_bounds__(256) k_upadj(const float* __restrict__ D, int ld, int coff, int h, int w, int C, int bilinear,
                                                float* __restrict__ dst, int VL, int PPB) {
+  pdl_enter();
   const int v = threadIdx.x % VL, slot = threadIdx.x / VL;
   item_loop<1>(blockIdx.x * PPB + slot, gridDim.x * PPB, h * w,
                [&](int p) {
@@ -1053,11 +1023,6 @@ __device__ __forceinline__ void d_upadj(const float* __restrict__ D, int ld, int
                  return upadj_read(D, ld, coff, h, w, i, j, v, bilinear);
                },
                [&](int p, float4 g) { st4(dst + static_cast<size_t>(p) * C + 4 * v, g); });
-}
-__global__ void __launch_bounds__(256) k_upadj(const float* __restrict__ D, int ld, int coff, int h, int w, int C, int bilinear,
-                                               float* __restrict__ dst, int VL, int PPB) {
-  pdl_enter();
-  d_upadj(D, ld, coff, h, w, C, bilinear, dst, VL, PPB);
 }
 void launch_upadj(const float* D, int ld, int coff, int h, int w, int C, int bilinear, float* dst, cudaStream_t s) {
   VecGeom g = vec_geom(C, static_cast<long long>(h) * w);
@@ -1243,33 +1208,29 @@ __device__ __forceinline__ void d_skinny_fwd_wide(const float* __restrict__ x, i
     block_reduce_atomic<2>(acc2, 1, 256, dst, wid);
   }
 }
-__device__ __forceinline__ void d_skinny_fwd(const float* __restrict__ x, int ldx, int x_rs, const float* __restrict__ w,
-                                             const float* __restrict__ b, int C, int N, int H, int W, float* __restrict__ y,
-                                             int mode, double* __restrict__ stats, int cw) {
+__global__ void __launch_bounds__(256) k_skinny_fwd(const float* __restrict__ x, int ldx, int x_rs, const float* __restrict__ w,
+                                                    const float* __restrict__ b, int C, int N, int H, int W,
+                                                    float* __restrict__ y, int mode, double* __restrict__ stats, int cw) {
+  pdl_enter();
   if (mode == 0 && C == 128) d_skinny_fwd_wide<32>(x, ldx, x_rs, w, b, N, H, W, y, stats, cw);
   else if (mode == 0 && C == 64) d_skinny_fwd_wide<16>(x, ldx, x_rs, w, b, N, H, W, y, stats, cw);
   else if (mode == 0 && C == 32) d_skinny_fwd_wide<8>(x, ldx, x_rs, w, b, N, H, W, y, stats, cw);
   else d_skinny_fwd_narrow(x, ldx, x_rs, w, b, C, N, H, W, y, mode, stats, cw);
 }
-__global__ void __launch_bounds__(256) k_skinny_fwd(const float* __restrict__ x, int ldx, int x_rs, const float* __restrict__ w,
-                                                    const float* __restrict__ b, int C, int N, int H, int W,
-                                                    float* __restrict__ y, int mode, double* __restrict__ stats, int cw) {
-  pdl_enter();
-  d_skinny_fwd(x, ldx, x_rs, w, b, C, N, H, W, y, mode, stats, cw);
-}
 void launch_skinny_fwd(const float* x, int ldx, int x_rs, const float* w, const float* b, int C, int N, int H,
                        int W, float* y, int mode, double* stats, cudaStream_t s, int cw) {
   const bool wide = mode == 0 && (C == 32 || C == 64 || C == 128);
-  const int PPB = wide ? 64 : 256 / skinny_lanes(C);   // pixels per block and trip of the path d_skinny_fwd takes
+  const int PPB = wide ? 64 : 256 / skinny_lanes(C);   // pixels per block and trip of the path k_skinny_fwd takes
   long long nb = (static_cast<long long>(H) * W + PPB - 1) / PPB;
   if (nb > kNumSms * 8) nb = kNumSms * 8;
   launch_red(k_skinny_fwd, static_cast<int>(nb), 256, 2 * 256 * sizeof(float4) + 2 * 4 * sizeof(double), s, x, ldx, x_rs, w, b, C, N, H, W,
                   y, mode, stats, cw > 0 ? cw : C);
 }
 
-__device__ __forceinline__ void d_skinny_bwd(const float* __restrict__ x, int ldx, int x_rs, const float* __restrict__ w, int C, int N,
+__global__ void k_skinny_bwd(const float* __restrict__ x, int ldx, int x_rs, const float* __restrict__ w, int C, int N,
                              int H, int W, const float* __restrict__ dy, const float* __restrict__ out_nchw, int mode,
                              float* __restrict__ dx, double* __restrict__ dw, double* __restrict__ db, int VL, int PPB, int cw) {
+  pdl_enter();
   const int v = threadIdx.x % VL, slot = threadIdx.x / VL;
   const int npix = H * W;
   float4 wv[4];
@@ -1315,12 +1276,6 @@ __device__ __forceinline__ void d_skinny_bwd(const float* __restrict__ x, int ld
                           N > 3 ? dw + 3 * C * kAccS : nullptr, db};
   const int wid[5] = {C, C, C, C, N};  // acc[4] (bias gradient) lives on lanes v == 0 only
   block_reduce_atomic<5>(acc, VL, PPB, dst, wid);
-}
-__global__ void k_skinny_bwd(const float* __restrict__ x, int ldx, int x_rs, const float* __restrict__ w, int C, int N,
-                             int H, int W, const float* __restrict__ dy, const float* __restrict__ out_nchw, int mode,
-                             float* __restrict__ dx, double* __restrict__ dw, double* __restrict__ db, int VL, int PPB, int cw) {
-  pdl_enter();
-  d_skinny_bwd(x, ldx, x_rs, w, C, N, H, W, dy, out_nchw, mode, dx, dw, db, VL, PPB, cw);
 }
 void launch_skinny_bwd(const float* x, int ldx, int x_rs, const float* w, int C, int N, int H, int W,
                        const float* dy, const float* out_nchw, int mode, float* dx, double* dw, double* db,

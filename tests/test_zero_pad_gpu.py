@@ -1,7 +1,7 @@
 """Zero padding on the engine (H100): every stage of one forward + backward against its fp64 reference at the engine's
 own inputs (tests/stage_ref.py under pad_refs.padding, the tolerances of tests/test_stages_gpu.py, every registered buffer
-NaN-filled first), exact-zero halos of every conv input and its bf16 twin, the notebook-facing API against fixtures of
-the unmodified reference (tests/golden/make_zero_pad.py), and the fallback of DIP_DEEP=1 to the launch-by-launch path."""
+NaN-filled first), exact-zero halos of every conv input and its bf16 twin, and the notebook-facing API against fixtures
+of the unmodified reference (tests/golden/make_zero_pad.py)."""
 import os
 
 import numpy as np
@@ -148,20 +148,6 @@ def run_runner(cfg, H, W, mode, task):
 def test_every_stage_runner_zero_pad(task, kind, H, W, mode):
     run_runner(cfg_of(kind), H, W, mode, task)
     TS.print_table()
-
-
-def test_deep_kernel_falls_back_for_zero_pad():
-    """DIP_DEEP=1 covers reflection halos only: a zero-padded 128-wide network keeps the launch-by-launch path and gives
-    bitwise the same output and gradients"""
-    cfg = cfg_of("cs4")
-    plan0, out0, g0 = run_direct(cfg, 64, 96, "tf32")
-    os.environ["DIP_DEEP"] = "1"
-    try:
-        plan1, out1, g1 = run_direct(cfg, 64, 96, "tf32")
-    finally:
-        os.environ.pop("DIP_DEEP", None)
-    assert plan0.num_launches() == plan1.num_launches()
-    assert torch.equal(out0, out1) and all(torch.equal(a, b) for a, b in zip(g0, g1))
 
 
 @pytest.mark.parametrize("prec", ["fp32", "tf32"])
