@@ -575,6 +575,7 @@ struct dip_plan {
   dip_net_desc desc;
   int H, W;
   int zero_pad = 0;   // dip_plan_opts.pad_mode == DIP_PAD_ZERO: conv-input halos hold zeros (Conv2d(padding=1))
+  int act_fun = DIP_ACT_LEAKY_RELU;   // dip_plan_opts.act_fun: the activation of every BN(+act) stage (kAct*)
   bool dry = false;
   uint8_t* ws = nullptr;
   size_t ws_bytes = 0;
@@ -1156,12 +1157,12 @@ static int fwd_level(dip_plan* P, int l, cudaStream_t s, int& nl) {
     nl += 2;
   }
   HBM_T(&P->timer, H_BN_ACT_WRITE, 1, (double)nd * ((double)v.h * v.w + (double)(v.h + 2) * (v.w + 2)) * sizeof(float), s,
-        launch_bn_act_write(v.raw_d1, nd, bn_ref(P, v.bn_d1), v.h, v.w, bf ? nullptr : v.P_d1, nd, 1, 1, s, Twin{v.P_d1_16, nd},
+        launch_bn_act_write(v.raw_d1, nd, bn_ref(P, v.bn_d1), v.h, v.w, bf ? nullptr : v.P_d1, nd, 1, 1, P->act_fun, s, Twin{v.P_d1_16, nd},
                             P->zero_pad));
   DIP_CHECK(v.d2.run_fprop(prec, P->params[v.d2.p_b], s));
   HBM_T(&P->timer, H_BN_ACT_WRITE, last ? 0 : 1,
         (double)nd * ((double)v.h * v.w + (last ? (double)v.h * v.w : (double)(v.h + 2) * (v.w + 2))) * sizeof(float), s,
-        launch_bn_act_write(v.raw_d2, nd, bn_ref(P, v.bn_d2), v.h, v.w, (bf && !last && P->lv[l + 1].ns != 4) ? nullptr : v.P_d2, nd, last ? 0 : 1, 1, s,
+        launch_bn_act_write(v.raw_d2, nd, bn_ref(P, v.bn_d2), v.h, v.w, (bf && !last && P->lv[l + 1].ns != 4) ? nullptr : v.P_d2, nd, last ? 0 : 1, 1, P->act_fun, s,
                             Twin{last ? nullptr : v.P_d2_16, nd}, P->zero_pad));   // (the 4-channel skip conv of the next level reads the fp32 tensor)
   nl += 4 + (prec == DIP_PRECISION_FP32 ? 2 : 0);
   if (!last) DIP_CHECK(fwd_level(P, l + 1, s, nl));
@@ -1169,16 +1170,16 @@ static int fwd_level(dip_plan* P, int l, cudaStream_t s, int& nl) {
   if (CS > 0) join_skip(P, s);
   CatArgs ca = cat_args(P, v, level_usrc(P, l));
   const double cat_in = ((double)v.cu * v.h * v.w + (double)CS * v.H * v.W) * sizeof(float);
-  HBM_T(&P->timer, H_CAT_STATS, v.bilinear, cat_in, s, launch_cat_stats(ca, v.bn_cat.fwd, s));
+  HBM_T(&P->timer, H_CAT_STATS, v.bilinear, cat_in, s, launch_cat_stats(ca, v.bn_cat.fwd, P->act_fun, s));
   HBM_T(&P->timer, H_CAT_WRITE, v.bilinear, cat_in + ((double)v.cu + CS) * (v.H + 2) * (v.W + 2) * sizeof(float), s,
-        launch_cat_write(ca, bn_ref(P, v.bn_cat), v.P_cat, s, Twin{v.P_cat16, v.cat_ld16}, P->zero_pad));
+        launch_cat_write(ca, bn_ref(P, v.bn_cat), v.P_cat, P->act_fun, s, Twin{v.P_cat16, v.cat_ld16}, P->zero_pad));
   DIP_CHECK(v.up.run_fprop(prec, P->params[v.up.p_b], s));
   HBM_T(&P->timer, H_BN_ACT_WRITE, 0, 2.0 * nu * v.H * v.W * sizeof(float), s,
-        launch_bn_act_write(v.raw_u, nu, bn_ref(P, v.bn_u), v.H, v.W, bf ? nullptr : v.A_u, nu, 0, 1, s, Twin{v.A_u16, nu}));
+        launch_bn_act_write(v.raw_u, nu, bn_ref(P, v.bn_u), v.H, v.W, bf ? nullptr : v.A_u, nu, 0, 1, P->act_fun, s, Twin{v.A_u16, nu}));
   DIP_CHECK(v.c11.run_fprop(prec, P->params[v.c11.p_b], s));
   if (l > 0 || nu != 128) {
     HBM_T(&P->timer, H_BN_ACT_WRITE, 0, 2.0 * nu * v.H * v.W * sizeof(float), s,
-          launch_bn_act_write(v.raw_v, nu, bn_ref(P, v.bn_v), v.H, v.W, v.U, nu, 0, 1, s));
+          launch_bn_act_write(v.raw_v, nu, bn_ref(P, v.bn_v), v.H, v.W, v.U, nu, 0, 1, P->act_fun, s));
     if (l == 0) {
       // level 0 narrower than 128 channels: the RGB head (models/skip.py:95-98) as a skinny 1x1 conv over the materialised
       // activation (the fused BN + head kernel is specialised for 128 channels = one warp per pixel)
@@ -1188,10 +1189,10 @@ static int fwd_level(dip_plan* P, int l, cudaStream_t s, int& nl) {
       nl += 1;
     }
   } else {
-    // top level: BN + LeakyReLU + RGB head + sigmoid in one pass; the 128-channel activation is never materialised
+    // top level: BN + activation + RGB head + sigmoid in one pass; the 128-channel activation is never materialised
     HeadRef hd{P->params[P->p_head_w], P->params[P->p_head_b], P->desc.out_channels, P->out_saved, P->desc.need_sigmoid != 0};
     HBM_T(&P->timer, H_BN_ACT_HEAD, 0, (128.0 + P->desc.out_channels) * v.H * v.W * sizeof(float), s,
-          launch_bn_act_head(v.raw_v, bn_ref(P, v.bn_v), v.H, v.W, hd, s));
+          launch_bn_act_head(v.raw_v, bn_ref(P, v.bn_v), v.H, v.W, hd, P->act_fun, s));
   }
   nl += 6 + (prec == DIP_PRECISION_FP32 ? 2 : 0);
   DIP_CUDA(cudaGetLastError());
@@ -1251,9 +1252,9 @@ static int bn_bwd(dip_plan* P, const float* raw, int ld_raw, BnLayer& b, int act
   if (src.kind == 1) gsrc = (src.zero_pad ? px : (double)(H + 2) * (W + 2)) * C4 + (src.ds != nullptr ? px * 4 * sizeof(float) : 0.0) + (src.add != nullptr ? px * C4 : 0.0);
   else if (src.kind == 2) gsrc = 4.0 * px * C4;
   else if (src.kind == 3) gsrc = px * 4 * sizeof(float);
-  HBM_T(&P->timer, H_BN_BWD_REDUCE, src.kind, px * C4 + gsrc, s, launch_bn_bwd_reduce(raw, ld_raw, r, act, src, H, W, b.bwd, s));
+  HBM_T(&P->timer, H_BN_BWD_REDUCE, src.kind, px * C4 + gsrc, s, launch_bn_bwd_reduce(raw, ld_raw, r, act, P->act_fun, src, H, W, b.bwd, s));
   HBM_T(&P->timer, H_BN_BWD_APPLY, src.kind + (zs != nullptr ? 4 : 0), px * C4 + gsrc + px * C4 * (zs != nullptr ? 2.0 : 1.0), s,
-        launch_bn_bwd_apply(raw, ld_raw, r, act, src, H, W, b.bwd, draw, zs, b.dbias, s, Twin{draw16, b.C}));
+        launch_bn_bwd_apply(raw, ld_raw, r, act, P->act_fun, src, H, W, b.bwd, draw, zs, b.dbias, s, Twin{draw16, b.C}));
   nl += 2;
   return 0;
 }
@@ -1463,12 +1464,19 @@ extern "C" {
 const char* dip_last_error(void) { return g_err.c_str(); }
 int dip_version(void) { return 100; }
 
-// options -> plan fields; NULL = defaults (reflection padding)
+static_assert(DIP_ACT_LEAKY_RELU == kActLeakyRelu && DIP_ACT_SWISH == kActSwish && DIP_ACT_ELU == kActElu &&
+                  DIP_ACT_NONE == kActNone, "the plan's act_fun is passed to the kernels as their kAct* kind");
+// options -> plan fields; NULL = defaults (reflection padding, LeakyReLU)
 static int apply_opts(dip_plan* P, const dip_plan_opts* opts) {
   const int pad = opts != nullptr ? opts->pad_mode : DIP_PAD_REFLECTION;
   if (pad != DIP_PAD_REFLECTION && pad != DIP_PAD_ZERO)
     return fail("dip-b200: pad_mode must be DIP_PAD_REFLECTION (0) or DIP_PAD_ZERO (1), got " + std::to_string(pad));
+  const int act = opts != nullptr ? opts->act_fun : DIP_ACT_LEAKY_RELU;
+  if (act < DIP_ACT_LEAKY_RELU || act > DIP_ACT_NONE)
+    return fail("dip-b200: act_fun must be DIP_ACT_LEAKY_RELU (0), DIP_ACT_SWISH (1), DIP_ACT_ELU (2) or DIP_ACT_NONE (3), got " +
+                std::to_string(act));
   P->zero_pad = pad == DIP_PAD_ZERO;
+  P->act_fun = act;
   return 0;
 }
 

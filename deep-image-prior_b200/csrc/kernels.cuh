@@ -11,6 +11,8 @@ namespace dip {
 static constexpr float kBnEps = 1e-5f;
 static constexpr long long kNumSms = 132;      // H100 SXM: grid caps of the grid-stride kernels (a few blocks per SM)
 static constexpr float kLreluSlope = 0.2f;
+// activation of every BN(+act) stage = models.skip's act_fun (models/common.py:76-92); the values are DIP_ACT_* of dip.h
+static constexpr int kActLeakyRelu = 0, kActSwish = 1, kActElu = 2, kActNone = 3;
 // fp64 accumulators are spread one per 128-byte line (stride in doubles): hundreds of blocks add to them at the end of
 // every reduction kernel: neighbouring channels must not share an L2 atomic unit, and each accumulator is split into
 // kAccR replicas (same-address atomics serialise) that readers add up
@@ -92,7 +94,7 @@ struct BnRef {
   float inv_n;         // 1 / (H*W)
 };
 
-// RGB head fused into the last BN+LeakyReLU stage: out[k][p] = sigmoid(b[k] + sum_c w[k][c] * act(bn(raw))[p][c])
+// RGB head fused into the last BN+activation stage: out[k][p] = sigmoid(b[k] + sum_c w[k][c] * act(bn(raw))[p][c])
 struct HeadRef {
   const float* w;      // [K][C] (torch [K][C][1][1])
   const float* b;      // [K]
@@ -111,14 +113,15 @@ void launch_input_pad(const float* z, const float* noise, float sigma, float* ds
 // generic per-channel sum / sum^2 of a plain NHWC tensor (SIMT-conv path and skinny convs)
 void launch_channel_stats(const float* x, int ld, int C, int npix, double* fwd, cudaStream_t s);
 
-// y = lrelu(bn(x)) written plain [H][W][ld_out] or reflection padded [(H+2)][(W+2)][ld_out]
+// y = f(bn(x)) written plain [H][W][ld_out] or reflection padded [(H+2)][(W+2)][ld_out]; f = the activation act_fun
+// (kAct*) when act != 0, else the identity
 // dst may be null when a bf16 twin is given (the tensor is then only read by tensor-core kernels)
 void launch_bn_act_write(const float* raw, int ld_in, BnRef bn, int H, int W, float* dst, int ld_out, int pad,
-                         int act, cudaStream_t s, Twin t16 = kNoTwin, int zero_pad = 0);
-// y = lrelu(bn(x)) consumed on the fly by the RGB head (C must be 128); y itself is not materialised
-void launch_bn_act_head(const float* raw, BnRef bn, int H, int W, HeadRef head, cudaStream_t s);
+                         int act, int act_fun, cudaStream_t s, Twin t16 = kNoTwin, int zero_pad = 0);
+// y = f(bn(x)) consumed on the fly by the RGB head (C must be 128); y itself is not materialised
+void launch_bn_act_head(const float* raw, BnRef bn, int H, int W, HeadRef head, int act_fun, cudaStream_t s);
 
-// Concat stage:  cat = [ up2x(U)(Cu ch) | lrelu(bn_s(raw_s))(Cs ch) ] at H x W (U is H/2 x W/2, plain, ld = Cu)
+// Concat stage:  cat = [ up2x(U)(Cu ch) | f(bn_s(raw_s))(Cs ch) ] at H x W (U is H/2 x W/2, plain, ld = Cu), f = act_fun
 struct CatArgs {
   const float* U;      // [H/2][W/2][Cu]
   const float* raw_s;  // [H][W][Cs]
@@ -126,9 +129,9 @@ struct CatArgs {
   int Cu, Cs, H, W;
   int bilinear;        // 1 bilinear (align_corners=False), 0 nearest
 };
-void launch_cat_stats(CatArgs a, double* fwd_cat, cudaStream_t s);
+void launch_cat_stats(CatArgs a, double* fwd_cat, int act_fun, cudaStream_t s);
 // dst = bn_cat(cat) with reflection pad: [(H+2)][(W+2)][Cu+Cs]
-void launch_cat_write(CatArgs a, BnRef bn_cat, float* dst, cudaStream_t s, Twin t16 = kNoTwin, int zero_pad = 0);
+void launch_cat_write(CatArgs a, BnRef bn_cat, float* dst, int act_fun, cudaStream_t s, Twin t16 = kNoTwin, int zero_pad = 0);
 
 // Gradient sources for the BN backward kernels
 struct GradSrc {
@@ -163,13 +166,14 @@ void launch_head_dlogit(const float* dout, const float* outv, int K, int npix, f
 void launch_input_grad(const float* gp, const float* ds, int ld, int C, int H, int W, float* dz, cudaStream_t s,
                        int zero_pad = 0);
 
-// BN(+LeakyReLU) backward. reduce: bwd[0..C) += sum dz, bwd[C..2C) += sum dz*xhat.
+// BN(+activation) backward. reduce: bwd[0..C) += sum dz, bwd[C..2C) += sum dz*xhat.
+// dz = f'(y) * gradient (act != 0; f = act_fun, y = the pre-activation, recomputed from raw) or the gradient itself.
 // apply: dx = gamma*rstd*(dz - mean(dz) - xhat*mean(dz*xhat)); writes draw plain [H][W][C];
 //        optionally a zero-stuffed copy zs [2H][2W][C] (only even positions written); dbias[c] += sum dx.
-void launch_bn_bwd_reduce(const float* raw, int ld_raw, BnRef bn, int act, GradSrc src, int H, int W, double* bwd,
-                          cudaStream_t s);
+void launch_bn_bwd_reduce(const float* raw, int ld_raw, BnRef bn, int act, int act_fun, GradSrc src, int H, int W,
+                          double* bwd, cudaStream_t s);
 // draw may be null when a bf16 twin is given
-void launch_bn_bwd_apply(const float* raw, int ld_raw, BnRef bn, int act, GradSrc src, int H, int W,
+void launch_bn_bwd_apply(const float* raw, int ld_raw, BnRef bn, int act, int act_fun, GradSrc src, int H, int W,
                          const double* bwd, float* draw, float* zs, double* dbias, cudaStream_t s, Twin t16 = kNoTwin);
 
 // In-net 'avg' downsampling (models/common.py:101-105: conv stride 1 + nn.AvgPool2d(2, 2)): y[i][j][c] = mean of the 2 x 2 block

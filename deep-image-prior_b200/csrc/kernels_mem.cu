@@ -4,7 +4,8 @@
 // (models/skip.py:41-100 built from models/common.py:76-124):
 //   input_pad        : net_input perturbation + nn.ReflectionPad2d(1)            (denoising.ipynb c10:12-13, common.py:117)
 //   bn_act_write     : nn.BatchNorm2d (training mode) + nn.LeakyReLU(0.2) + nn.ReflectionPad2d(1)   (common.py:96,82,117)
-//                      (pad != 'reflection': the zero halo of Conv2d(padding=1) instead, in every halo writer / fold below)
+//                      (pad != 'reflection': the zero halo of Conv2d(padding=1) instead, in every halo writer / fold below;
+//                       act_fun 'Swish' / 'ELU' / 'none' (common.py:76-92) instead of LeakyReLU in every BN(+act) kernel)
 //   bn_act_head      : last BN + LeakyReLU + 1x1 conv 128->3 + nn.Sigmoid in one pass (skip.py:90-98)
 //   cat_stats/write  : nn.Upsample(x2) + Concat + nn.BatchNorm2d(132) + pad     (skip.py:81,50-55; common.py:19-39)
 //   bn_bwd_*/cat_bwd_*: autograd adjoints of the above, with the producer of the incoming gradient fused in
@@ -18,6 +19,7 @@
 #include <stdlib.h>
 
 #include <map>
+#include <type_traits>
 #include <utility>
 
 
@@ -67,8 +69,46 @@ __device__ __forceinline__ uint16_t bf16_bits(float x) {
 }
 __device__ __forceinline__ float4 f4zero() { return make_float4(0.f, 0.f, 0.f, 0.f); }
 __device__ __forceinline__ float f4dot(float4 a, float4 b) { return a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w; }
-__device__ __forceinline__ float lrelu(float y) { return y > 0.f ? y : kLreluSlope * y; }
-__device__ __forceinline__ float4 lrelu4(float4 y) { return make_float4(lrelu(y.x), lrelu(y.y), lrelu(y.z), lrelu(y.w)); }
+// The activation f of every BN(+act) stage and its adjoint g * f'(y), both of the fp32 pre-activation y = fma(x, scale, shift)
+// (ACT: kAct*).  Swish's sigmoid is 1 / (1 + e^-y), which tends to 0 or 1 for large |y| without an inf / inf or 0 * inf.
+template <int ACT>
+__device__ __forceinline__ float act_fwd(float y) {
+  if constexpr (ACT == kActSwish) return y * (1.f / (1.f + expf(-y)));
+  else if constexpr (ACT == kActElu) return y > 0.f ? y : expm1f(y);
+  else if constexpr (ACT == kActNone) return y;
+  else return y > 0.f ? y : kLreluSlope * y;
+}
+template <int ACT>
+__device__ __forceinline__ float act_bwd(float y, float g) {
+  if constexpr (ACT == kActSwish) {
+    const float s = 1.f / (1.f + expf(-y));
+    return g * (s * (1.f + y * (1.f - s)));
+  } else if constexpr (ACT == kActElu) {
+    return y > 0.f ? g : g * expf(y);
+  } else if constexpr (ACT == kActNone) {
+    return g;
+  } else {
+    return y > 0.f ? g : kLreluSlope * g;
+  }
+}
+template <int ACT>
+__device__ __forceinline__ float4 act_fwd4(float4 y) {
+  return make_float4(act_fwd<ACT>(y.x), act_fwd<ACT>(y.y), act_fwd<ACT>(y.z), act_fwd<ACT>(y.w));
+}
+template <int ACT>
+__device__ __forceinline__ float4 act_bwd4(float4 y, float4 g) {
+  return make_float4(act_bwd<ACT>(y.x, g.x), act_bwd<ACT>(y.y, g.y), act_bwd<ACT>(y.z, g.z), act_bwd<ACT>(y.w, g.w));
+}
+// the kernel instantiation for a plan's activation kind: pick(std::integral_constant<int, ACT>) returns it
+template <class Pick>
+static auto act_pick(int act_fun, Pick pick) {
+  switch (act_fun) {
+    case kActSwish: return pick(std::integral_constant<int, kActSwish>());
+    case kActElu: return pick(std::integral_constant<int, kActElu>());
+    case kActNone: return pick(std::integral_constant<int, kActNone>());
+    default: return pick(std::integral_constant<int, kActLeakyRelu>());
+  }
+}
 __device__ __forceinline__ float4 shfl_xor4(float4 a, int o) {
   return make_float4(__shfl_xor_sync(0xffffffffu, a.x, o), __shfl_xor_sync(0xffffffffu, a.y, o),
                      __shfl_xor_sync(0xffffffffu, a.z, o), __shfl_xor_sync(0xffffffffu, a.w, o));
@@ -323,7 +363,9 @@ void launch_channel_stats(const float* x, int ld, int C, int npix, double* fwd, 
 
 // ------------------------------------------------------------------------------------------------ bn_act_write
 // ZP: with pad, the halo cells are written as 0 (their load reads the nearest interior pixel, whose value is discarded)
-template <bool ZP>
+// ACT: the activation applied when act != 0 (kAct*; like ZP a template parameter, so the LeakyReLU instantiations of
+// this kernel and of the other BN(+act) kernels below are the unchanged code)
+template <bool ZP, int ACT>
 __global__ void __launch_bounds__(256) k_bn_act_write(const float* __restrict__ raw, int ld_in, BnRef bn, int H, int W,
                                                       float* __restrict__ dst, int ld_out, int pad, int act, int VL,
                                                       int PPB, Twin t16) {
@@ -340,7 +382,7 @@ __global__ void __launch_bounds__(256) k_bn_act_write(const float* __restrict__ 
                },
                [&](int p, float4 x) {
                  float4 y = bn_apply(cf, x);
-                 if (act) y = lrelu4(y);
+                 if (act) y = act_fwd4<ACT>(y);
                  if (ZP && pad) {
                    const int yo = p / Wo, xo = p - yo * Wo;
                    if (yo == 0 || yo == Ho - 1 || xo == 0 || xo == Wo - 1) y = f4zero();
@@ -350,14 +392,18 @@ __global__ void __launch_bounds__(256) k_bn_act_write(const float* __restrict__ 
                });
 }
 void launch_bn_act_write(const float* raw, int ld_in, BnRef bn, int H, int W, float* dst, int ld_out, int pad,
-                         int act, cudaStream_t s, Twin t16, int zero_pad) {
+                         int act, int act_fun, cudaStream_t s, Twin t16, int zero_pad) {
   VecGeom g = vec_geom(bn.C, static_cast<long long>(H + 2 * pad) * (W + 2 * pad));
-  auto kernel = zero_pad && pad ? k_bn_act_write<true> : k_bn_act_write<false>;
+  auto kernel = act_pick(act_fun, [&](auto a) {
+    constexpr int A = decltype(a)::value;
+    return zero_pad && pad ? k_bn_act_write<true, A> : k_bn_act_write<false, A>;
+  });
   fit_grid(g, kernel, 0);
   launch_k(kernel, dim3(g.blocks), dim3(g.threads), 0, s, 1, raw, ld_in, bn, H, W, dst, ld_out, pad, act, g.VL, g.PPB, t16);
 }
 
-// BN + LeakyReLU + RGB head + sigmoid: one warp per pixel (C = 128 -> 32 lanes x float4), nothing but out is written.
+// BN + activation + RGB head + sigmoid: one warp per pixel (C = 128 -> 32 lanes x float4), nothing but out is written.
+template <int ACT>
 __global__ void __launch_bounds__(256) k_bn_act_head(const float* __restrict__ raw, BnRef bn, int npix, HeadRef head) {
   pdl_enter();
   const int lane = threadIdx.x & 31, wslot = threadIdx.x >> 5;
@@ -369,7 +415,7 @@ __global__ void __launch_bounds__(256) k_bn_act_head(const float* __restrict__ r
   item_loop<DIP_U_HEAD>(blockIdx.x * 8 + wslot, gridDim.x * 8, npix,
                [&](int p) { return ld4(raw + static_cast<size_t>(p) * 128 + 4 * lane); },
                [&](int p, float4 x) {
-                 const float4 y = lrelu4(bn_apply(cf, x));
+                 const float4 y = act_fwd4<ACT>(bn_apply(cf, x));
                  float d[4];
 #pragma unroll
                  for (int k = 0; k < 4; ++k) d[k] = f4dot(y, w[k]);
@@ -391,11 +437,12 @@ __global__ void __launch_bounds__(256) k_bn_act_head(const float* __restrict__ r
                  }
                });
 }
-void launch_bn_act_head(const float* raw, BnRef bn, int H, int W, HeadRef head, cudaStream_t s) {
+void launch_bn_act_head(const float* raw, BnRef bn, int H, int W, HeadRef head, int act_fun, cudaStream_t s) {
   const int npix = H * W;
   int blocks = (npix + 7) / 8;
   if (blocks > kNumSms * 8) blocks = kNumSms * 8;
-  launch_k(k_bn_act_head, dim3(blocks), dim3(256), 0, s, 1, raw, bn, npix, head);
+  auto kernel = act_pick(act_fun, [](auto a) { return k_bn_act_head<decltype(a)::value>; });
+  launch_k(kernel, dim3(blocks), dim3(256), 0, s, 1, raw, bn, npix, head);
 }
 
 // ------------------------------------------------------------------------------------------------ concat stage
@@ -411,7 +458,8 @@ __device__ __forceinline__ CatLane cat_lane(const CatArgs& a, int v) {
   l.bs = bn_coef<1>(a.bn_s, l.is_up ? -1 : v - a.Cu / 4);
   return l;
 }
-// out[0..3] = pre-BN concat values at (2si,2sj), (2si,2sj+1), (2si+1,2sj), (2si+1,2sj+1)
+// out[0..3] = pre-BN concat values at (2si,2sj), (2si,2sj+1), (2si+1,2sj), (2si+1,2sj+1) (skip branch: activation ACT)
+template <int ACT>
 __device__ __forceinline__ void cat_quad(const CatArgs& a, const CatLane& l, int si, int sj, int v, float4 (&out)[4]) {
   const int h = a.H >> 1, w = a.W >> 1;
   if (l.is_up) {
@@ -443,11 +491,12 @@ __device__ __forceinline__ void cat_quad(const CatArgs& a, const CatLane& l, int
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
       const int i = 2 * si + (q >> 1), j = 2 * sj + (q & 1);
-      out[q] = lrelu4(bn_apply(l.bs, ld4(base + (static_cast<size_t>(i) * a.W + j) * a.Cs)));
+      out[q] = act_fwd4<ACT>(bn_apply(l.bs, ld4(base + (static_cast<size_t>(i) * a.W + j) * a.Cs)));
     }
   }
 }
 
+template <int ACT>
 __global__ void __launch_bounds__(256, DIP_CAT_MINBLOCKS) k_cat_stats(CatArgs a, double* __restrict__ fwd, int VL, int PPB) {
   pdl_enter();
   const int v = threadIdx.x % VL, slot = threadIdx.x / VL;
@@ -457,7 +506,7 @@ __global__ void __launch_bounds__(256, DIP_CAT_MINBLOCKS) k_cat_stats(CatArgs a,
   for (int p = slot < PPB ? blockIdx.x * PPB + slot : nsrc; p < nsrc; p += gridDim.x * PPB) {
     const int si = p / w, sj = p - si * w;
     float4 q[4];
-    cat_quad(a, l, si, sj, v, q);
+    cat_quad<ACT>(a, l, si, sj, v, q);
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       acc[0] = f4add(acc[0], q[e]);
@@ -468,10 +517,11 @@ __global__ void __launch_bounds__(256, DIP_CAT_MINBLOCKS) k_cat_stats(CatArgs a,
   const int wid[2] = {a.Cu + a.Cs, a.Cu + a.Cs};
   block_reduce_atomic<2>(acc, VL, PPB, dst, wid);
 }
-void launch_cat_stats(CatArgs a, double* fwd_cat, cudaStream_t s) {
+void launch_cat_stats(CatArgs a, double* fwd_cat, int act_fun, cudaStream_t s) {
   VecGeom g = vec_geom(a.Cu + a.Cs, static_cast<long long>(a.H / 2) * (a.W / 2));
-  fit_grid(g, k_cat_stats, red_bytes(g, 2));
-  launch_red(k_cat_stats, g.blocks, g.threads, red_bytes(g, 2), s, a, fwd_cat, g.VL, g.PPB);
+  auto kernel = act_pick(act_fun, [](auto x) { return k_cat_stats<decltype(x)::value>; });
+  fit_grid(g, kernel, red_bytes(g, 2));
+  launch_red(kernel, g.blocks, g.threads, red_bytes(g, 2), s, a, fwd_cat, g.VL, g.PPB);
 }
 
 // store the value of interior pixel (i, j) at its padded position and at every halo position that mirrors it
@@ -497,7 +547,7 @@ __device__ __forceinline__ void store_with_halo(float* __restrict__ dst, int ld,
     }
 }
 
-template <bool ZP>
+template <bool ZP, int ACT>
 __global__ void __launch_bounds__(256, DIP_CAT_MINBLOCKS) k_cat_write(CatArgs a, BnRef bn_cat, float* __restrict__ dst, int VL, int PPB, Twin t16) {
   pdl_enter();
   const int v = threadIdx.x % VL, slot = threadIdx.x / VL;
@@ -508,15 +558,18 @@ __global__ void __launch_bounds__(256, DIP_CAT_MINBLOCKS) k_cat_write(CatArgs a,
   for (int p = slot < PPB ? blockIdx.x * PPB + slot : nsrc; p < nsrc; p += gridDim.x * PPB) {
     const int si = p / w, sj = p - si * w;
     float4 q[4];
-    cat_quad(a, l, si, sj, v, q);
+    cat_quad<ACT>(a, l, si, sj, v, q);
 #pragma unroll
     for (int e = 0; e < 4; ++e)
       store_with_halo<ZP>(dst, ld, a.H, a.W, 2 * si + (e >> 1), 2 * sj + (e & 1), v, bn_apply(cf, q[e]), t16);
   }
 }
-void launch_cat_write(CatArgs a, BnRef bn_cat, float* dst, cudaStream_t s, Twin t16, int zero_pad) {
+void launch_cat_write(CatArgs a, BnRef bn_cat, float* dst, int act_fun, cudaStream_t s, Twin t16, int zero_pad) {
   VecGeom g = vec_geom(a.Cu + a.Cs, static_cast<long long>(a.H / 2) * (a.W / 2));
-  auto kernel = zero_pad ? k_cat_write<true> : k_cat_write<false>;
+  auto kernel = act_pick(act_fun, [&](auto x) {
+    constexpr int A = decltype(x)::value;
+    return zero_pad ? k_cat_write<true, A> : k_cat_write<false, A>;
+  });
   fit_grid(g, kernel, 0);
   launch_k(kernel, dim3(g.blocks), dim3(g.threads), 0, s, 1, a, bn_cat, dst, g.VL, g.PPB, t16);
 }
@@ -622,10 +675,6 @@ __device__ __forceinline__ float4 head_grad(const SrcRegs& sr, float4 d) {
   r = f4fma(d.z, sr.w[2], r);
   r = f4fma(d.w, sr.w[3], r);
   return r;
-}
-__device__ __forceinline__ float4 lrelu_bwd4(float4 y, float4 g) {
-  return make_float4(y.x > 0.f ? g.x : kLreluSlope * g.x, y.y > 0.f ? g.y : kLreluSlope * g.y,
-                     y.z > 0.f ? g.z : kLreluSlope * g.z, y.w > 0.f ? g.w : kLreluSlope * g.w);
 }
 
 // Row-segment loop for kernels whose gradient source is a reflection-pad fold (padded dgrad output): a block takes units of
@@ -763,8 +812,9 @@ void launch_input_grad(const float* gp, const float* ds, int ld, int C, int H, i
   dim3 grid((W + 31) / 32, H), block(32, 8);
   launch_k(zero_pad ? k_input_grad<true> : k_input_grad<false>, dim3(grid), dim3(block), 0, s, 1, gp, ds, ld, C, H, W, dz);
 }
-// ZP applies to KIND 1 only: the padded gradient's halo is dropped instead of folded (zero-padding adjoint)
-template <int KIND, bool ZP = false>
+// ZP applies to KIND 1 only: the padded gradient's halo is dropped instead of folded (zero-padding adjoint).
+// ACT: the activation's adjoint (act != 0), from the pre-activation recomputed from raw, as in the forward.
+template <int KIND, bool ZP = false, int ACT = kActLeakyRelu>
 __device__ __forceinline__ void d_bn_bwd_reduce(const float* __restrict__ raw, int ld_raw, BnRef bn, int act, GradSrc src,
                                                        int H, int W, double* __restrict__ bwd, int VL, int PPB) {
   const int v = threadIdx.x % VL, slot = threadIdx.x / VL;
@@ -777,7 +827,7 @@ __device__ __forceinline__ void d_bn_bwd_reduce(const float* __restrict__ raw, i
                          [&](int i, int j, int u) { fold_item_load(src, raw, ld_raw, W, i, j, v, it[u]); },
                          [&](int i, int j, int u) {
                            float4 dz = fold_item_grad<ZP>(src, sr, H, W, i, j, v, it[u]);
-                           if (act) dz = lrelu_bwd4(bn_apply(cf, it[u].x), dz);
+                           if (act) dz = act_bwd4<ACT>(bn_apply(cf, it[u].x), dz);
                            acc[0] = f4add(acc[0], dz);
                            acc[1] = f4mla(dz, bn_xhat(cf, it[u].x), acc[1]);
                          });
@@ -793,7 +843,7 @@ __device__ __forceinline__ void d_bn_bwd_reduce(const float* __restrict__ raw, i
       },
       [&](int, const RedItem& it) {
         float4 dz = KIND == 3 ? head_grad(sr, it.g) : it.g;
-        if (act) dz = lrelu_bwd4(bn_apply(cf, it.x), dz);
+        if (act) dz = act_bwd4<ACT>(bn_apply(cf, it.x), dz);
         acc[0] = f4add(acc[0], dz);
         acc[1] = f4mla(dz, bn_xhat(cf, it.x), acc[1]);
       });
@@ -801,26 +851,29 @@ __device__ __forceinline__ void d_bn_bwd_reduce(const float* __restrict__ raw, i
   const int wid[2] = {bn.C, bn.C};
   block_reduce_atomic<2>(acc, VL, PPB, dst, wid);
 }
-template <int KIND, bool ZP = false>
+template <int KIND, bool ZP = false, int ACT = kActLeakyRelu>
 __global__ void __launch_bounds__(256, (KIND == 0 || KIND == 2) ? 3 : 2) k_bn_bwd_reduce(const float* __restrict__ raw, int ld_raw, BnRef bn, int act, GradSrc src,
                                                        int H, int W, double* __restrict__ bwd, int VL, int PPB) {
   pdl_enter();
-  d_bn_bwd_reduce<KIND, ZP>(raw, ld_raw, bn, act, src, H, W, bwd, VL, PPB);
+  d_bn_bwd_reduce<KIND, ZP, ACT>(raw, ld_raw, bn, act, src, H, W, bwd, VL, PPB);
 }
-void launch_bn_bwd_reduce(const float* raw, int ld_raw, BnRef bn, int act, GradSrc src, int H, int W, double* bwd,
-                          cudaStream_t s) {
+void launch_bn_bwd_reduce(const float* raw, int ld_raw, BnRef bn, int act, int act_fun, GradSrc src, int H, int W,
+                          double* bwd, cudaStream_t s) {
   VecGeom g = vec_geom(bn.C, static_cast<long long>(H) * W);
   const size_t sm = red_bytes(g, 2);
-  auto kernel = src.kind == 0 ? k_bn_bwd_reduce<0>
-              : src.kind == 1 ? (src.zero_pad ? k_bn_bwd_reduce<1, true> : k_bn_bwd_reduce<1>)
-              : src.kind == 2 ? k_bn_bwd_reduce<2> : k_bn_bwd_reduce<3>;
+  auto kernel = act_pick(act_fun, [&](auto a) {
+    constexpr int A = decltype(a)::value;
+    return src.kind == 0 ? k_bn_bwd_reduce<0, false, A>
+         : src.kind == 1 ? (src.zero_pad ? k_bn_bwd_reduce<1, true, A> : k_bn_bwd_reduce<1, false, A>)
+         : src.kind == 2 ? k_bn_bwd_reduce<2, false, A> : k_bn_bwd_reduce<3, false, A>;
+  });
   fit_grid(g, kernel, sm);
   launch_red(kernel, g.blocks, g.threads, sm, s, raw, ld_raw, bn, act, src, H, W, bwd, g.VL, g.PPB);
 }
 
 // apply pass; for the head source (KIND 3) it also accumulates the head's own gradients:
 //   dW_head[k][c] += dl[k] * act(bn(raw))[c],  db_head[k] += dl[k]
-template <int KIND, bool ZP = false>
+template <int KIND, bool ZP = false, int ACT = kActLeakyRelu>
 __global__ void __launch_bounds__(256, KIND == 2 ? 3 : 2) k_bn_bwd_apply(const float* __restrict__ raw, int ld_raw, BnRef bn, int act, GradSrc src,
                                                       int H, int W, const double* __restrict__ bwd, float* __restrict__ draw,
                                                       float* __restrict__ zs, double* __restrict__ dbias, int VL, int PPB, Twin t16) {
@@ -841,7 +894,7 @@ __global__ void __launch_bounds__(256, KIND == 2 ? 3 : 2) k_bn_bwd_apply(const f
                          [&](int i, int j, int u) { fold_item_load(src, raw, ld_raw, W, i, j, v, it[u]); },
                          [&](int i, int j, int u) {
                            float4 dz = fold_item_grad<ZP>(src, sr, H, W, i, j, v, it[u]);
-                           if (act) dz = lrelu_bwd4(bn_apply(cf, it[u].x), dz);
+                           if (act) dz = act_bwd4<ACT>(bn_apply(cf, it[u].x), dz);
                            const float4 xh = bn_xhat(cf, it[u].x);
                            float4 dx;
                            dx.x = cf.scale.x * (dz.x - m1.x - xh.x * m2.x);
@@ -867,7 +920,7 @@ __global__ void __launch_bounds__(256, KIND == 2 ? 3 : 2) k_bn_bwd_apply(const f
         float4 dz = KIND == 3 ? head_grad(sr, it.g) : it.g;
         const float4 y = bn_apply(cf, it.x);
         if constexpr (KIND == 3) {
-          const float4 u = act ? lrelu4(y) : y;
+          const float4 u = act ? act_fwd4<ACT>(y) : y;
 #pragma unroll
           acc[1] = f4fma(it.g.x, u, acc[1]);
           acc[2] = f4fma(it.g.y, u, acc[2]);
@@ -875,7 +928,7 @@ __global__ void __launch_bounds__(256, KIND == 2 ? 3 : 2) k_bn_bwd_apply(const f
           acc[4] = f4fma(it.g.w, u, acc[4]);
           if (v == 0) acc[5] = f4add(acc[5], it.g);
         }
-        if (act) dz = lrelu_bwd4(y, dz);
+        if (act) dz = act_bwd4<ACT>(y, dz);
         const float4 xh = bn_xhat(cf, it.x);
         float4 dx;
         dx.x = cf.scale.x * (dz.x - m1.x - xh.x * m2.x);
@@ -902,13 +955,16 @@ __global__ void __launch_bounds__(256, KIND == 2 ? 3 : 2) k_bn_bwd_apply(const f
     block_reduce_atomic<K>(acc, VL, PPB, dst, wid);
   }
 }
-void launch_bn_bwd_apply(const float* raw, int ld_raw, BnRef bn, int act, GradSrc src, int H, int W,
+void launch_bn_bwd_apply(const float* raw, int ld_raw, BnRef bn, int act, int act_fun, GradSrc src, int H, int W,
                          const double* bwd, float* draw, float* zs, double* dbias, cudaStream_t s, Twin t16) {
   VecGeom g = vec_geom(bn.C, static_cast<long long>(H) * W);
   const size_t sm = red_bytes(g, src.kind == 3 ? 6 : 1);
-  auto kernel = src.kind == 0 ? k_bn_bwd_apply<0>
-              : src.kind == 1 ? (src.zero_pad ? k_bn_bwd_apply<1, true> : k_bn_bwd_apply<1>)
-              : src.kind == 2 ? k_bn_bwd_apply<2> : k_bn_bwd_apply<3>;
+  auto kernel = act_pick(act_fun, [&](auto a) {
+    constexpr int A = decltype(a)::value;
+    return src.kind == 0 ? k_bn_bwd_apply<0, false, A>
+         : src.kind == 1 ? (src.zero_pad ? k_bn_bwd_apply<1, true, A> : k_bn_bwd_apply<1, false, A>)
+         : src.kind == 2 ? k_bn_bwd_apply<2, false, A> : k_bn_bwd_apply<3, false, A>;
+  });
   fit_grid(g, kernel, sm);
   launch_red(kernel, g.blocks, g.threads, sm, s, raw, ld_raw, bn, act, src, H, W, bwd, draw, zs, dbias, g.VL, g.PPB, t16);
 }

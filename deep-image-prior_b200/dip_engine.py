@@ -20,6 +20,14 @@ PRECISION_BF16 = 2
 PAD_REFLECTION = 0   # dip_plan_opts.pad_mode: nn.ReflectionPad2d(1) before every 3x3 conv (models.skip pad='reflection')
 PAD_ZERO = 1         # Conv2d(padding=1): every other value of models.skip's `pad` (reference: models/common.py:114-120)
 
+# dip_plan_opts.act_fun: models.skip's act_fun string (reference: models/common.py:76-92), the activation behind every
+# BatchNorm except the concat's
+ACT_LEAKY_RELU = 0   # 'LeakyReLU': nn.LeakyReLU(0.2)
+ACT_SWISH = 1        # 'Swish': x * sigmoid(x)
+ACT_ELU = 2          # 'ELU': nn.ELU() (alpha = 1)
+ACT_NONE = 3         # 'none': nn.Sequential(), the identity
+ACT_FUNS = {"LeakyReLU": ACT_LEAKY_RELU, "Swish": ACT_SWISH, "ELU": ACT_ELU, "none": ACT_NONE}
+
 
 class NetDesc(ctypes.Structure):
     _fields_ = [
@@ -41,8 +49,8 @@ class NetDesc(ctypes.Structure):
 
 
 class PlanOpts(ctypes.Structure):
-    """dip_plan_opts (include/dip.h)"""
-    _fields_ = [("pad_mode", ctypes.c_int)]
+    """dip_plan_opts (include/dip.h): PlanOpts(pad_mode, act_fun); a field left out is 0 (reflection, LeakyReLU)"""
+    _fields_ = [("pad_mode", ctypes.c_int), ("act_fun", ctypes.c_int)]
 
 
 _lib = None
@@ -153,15 +161,17 @@ class Plan:
 
     def __init__(self, in_channels, out_channels, num_scales, channels, skip_channels, bilinear, H, W,
                  precision=PRECISION_TF32, device=None, need_sigmoid=True, input_grad=False, channels_up=None,
-                 downsample_mode="stride", pad="reflection"):
+                 downsample_mode="stride", pad="reflection", act="LeakyReLU"):
         """channels / skip_channels: one width for every scale, or per-scale sequences (num_channels_down / num_channels_skip
         of models.skip; channels_up = num_channels_up, default = channels).  pad: 'reflection' or 'zero' (the padding of
-        every 3x3 conv)."""
+        every 3x3 conv).  act: 'LeakyReLU', 'Swish', 'ELU' or 'none' (models.skip's act_fun)."""
         L = lib()
         if pad not in ("reflection", "zero"):
             raise ValueError("dip-b200: Plan(pad=...) must be 'reflection' or 'zero', not %r" % (pad,))
-        self.opts = PlanOpts(PAD_REFLECTION if pad == "reflection" else PAD_ZERO)
-        self.pad = pad
+        if not isinstance(act, str) or act not in ACT_FUNS:
+            raise ValueError("dip-b200: Plan(act=...) must be one of %s, not %r" % (", ".join(map(repr, ACT_FUNS)), act))
+        self.opts = PlanOpts(PAD_REFLECTION if pad == "reflection" else PAD_ZERO, ACT_FUNS[act])
+        self.pad, self.act = pad, act
         per_scale = None
         if isinstance(channels, (list, tuple)) or isinstance(skip_channels, (list, tuple)) or channels_up is not None:
             as_list = lambda x: list(x) if isinstance(x, (list, tuple)) else [x] * num_scales   # noqa: E731

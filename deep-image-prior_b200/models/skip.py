@@ -104,13 +104,14 @@ class SkipNet(nn.Sequential):
         import dip_engine as de
         spec = self._dip_spec
         H, W = key[0], key[1]
-        pkey = (H, W, str(z.device), prec, key[4], spec.get('pad', 'reflection'))
+        pkey = (H, W, str(z.device), prec, key[4], spec.get('pad', 'reflection'), spec.get('act_fun', 'LeakyReLU'))
         plan = self._dip_plans.get(pkey)
         if plan is None:
             plan = de.Plan(spec['in_channels'], spec['out_channels'], spec['num_scales'], spec['channels'],
                            spec['skip_channels'], spec['bilinear'], H, W, precision=prec, device=z.device,
                            need_sigmoid=spec['need_sigmoid'], input_grad=key[4], channels_up=spec.get('channels_up'),
-                           downsample_mode=spec.get('downsample_mode', 'stride'), pad=spec.get('pad', 'reflection'))
+                           downsample_mode=spec.get('downsample_mode', 'stride'), pad=spec.get('pad', 'reflection'),
+                           act=spec.get('act_fun', 'LeakyReLU'))
             self._dip_plans[pkey] = plan
         params = list(self.parameters())
         for p in params:
@@ -263,8 +264,8 @@ def skip(num_input_channels=2, num_output_channels=3,
         why = 'filter sizes must be 3/3/1'
     elif set(downsample_mode) not in ({'stride'}, {'avg'}):
         why = "downsample_mode must be 'stride' or 'avg' (at every scale)"
-    elif act_fun != 'LeakyReLU':
-        why = "act_fun must be 'LeakyReLU'"
+    elif not (isinstance(act_fun, str) and act_fun in ('LeakyReLU', 'Swish', 'ELU', 'none')):
+        why = "act_fun must be 'LeakyReLU', 'Swish', 'ELU' or 'none' (a module class is not accelerated)"
     elif not (need_bias and need1x1_up):
         why = 'need_bias and need1x1_up must be True'
     elif any(m not in ('bilinear', 'nearest') for m in upsample_mode):
@@ -281,6 +282,7 @@ def skip(num_input_channels=2, num_output_channels=3,
                              # models/common.py:conv: only pad == 'reflection' inserts ReflectionPad2d, any other value
                              # is Conv2d(padding=(k-1)//2), i.e. zero padding
                              pad='reflection' if pad == 'reflection' else 'zero',
+                             act_fun=act_fun,
                              bilinear=(upsample_mode[0] == 'bilinear' if len(set(upsample_mode)) == 1
                                        else [m == 'bilinear' for m in upsample_mode]))
     else:

@@ -63,14 +63,22 @@ size_t dip_plan_workspace_bytes(const dip_net_desc* desc, int H, int W);
 int dip_plan_create(const dip_net_desc* desc, int H, int W, void* workspace, size_t workspace_bytes,
                     dip_plan** out);
 
-/* Plan options beyond dip_net_desc.  pad_mode = the `pad` argument of models.skip (reference: models/common.py:114-120):
- * DIP_PAD_REFLECTION inserts nn.ReflectionPad2d before every 3x3 conv; any other value of `pad` gives
- * Conv2d(padding=1), i.e. DIP_PAD_ZERO.  Both modes need the same workspace.  Other values are rejected. */
+/* Plan options beyond dip_net_desc: the struct is {pad_mode, act_fun}, and a zero-initialised one (or opts == NULL) is
+ * reflection padding with LeakyReLU.
+ * pad_mode = the `pad` argument of models.skip (reference: models/common.py:114-120): DIP_PAD_REFLECTION inserts
+ * nn.ReflectionPad2d before every 3x3 conv; any other value of `pad` gives Conv2d(padding=1), i.e. DIP_PAD_ZERO.
+ * act_fun = the `act_fun` string of models.skip (reference: models/common.py:76-92), the activation behind every
+ * BatchNorm except the concat's: 'LeakyReLU' = nn.LeakyReLU(0.2), 'Swish' = x * sigmoid(x), 'ELU' = nn.ELU() (alpha 1),
+ * 'none' = the identity.
+ * Every combination needs the same workspace.  Other values are rejected (dip_last_error() names the field). */
 enum { DIP_PAD_REFLECTION = 0, DIP_PAD_ZERO = 1 };
+enum { DIP_ACT_LEAKY_RELU = 0, DIP_ACT_SWISH = 1, DIP_ACT_ELU = 2, DIP_ACT_NONE = 3 };
 typedef struct {
   int pad_mode;          /* DIP_PAD_*                                                                     */
+  int act_fun;           /* DIP_ACT_*                                                                     */
 } dip_plan_opts;
-/* as dip_plan_workspace_bytes / dip_plan_create; opts may be NULL (= reflection padding, what the two calls above use) */
+/* as dip_plan_workspace_bytes / dip_plan_create; opts may be NULL (= reflection padding and LeakyReLU, what the two calls
+ * above use) */
 size_t dip_plan_workspace_bytes_opts(const dip_net_desc* desc, int H, int W, const dip_plan_opts* opts);
 int dip_plan_create_opts(const dip_net_desc* desc, int H, int W, const dip_plan_opts* opts, void* workspace,
                          size_t workspace_bytes, dip_plan** out);
