@@ -994,6 +994,7 @@ static int build_plan(dip_plan* P, Arena& A) {
     for (ConvOp* op : P->convs) if (op->do_wgrad) { tot += (op->wacc_elems() + 63) & ~size_t(63); P->n_unpack++; }
     P->wacc_base = A.get<float>(tot);
     P->wacc_bytes = tot * sizeof(float);
+    if (P->wacc_base != nullptr) reg("wacc", P->wacc_base, 1, 1, (int)tot, (int)tot);   // (tests NaN-fill it)
     size_t off = 0;
     for (ConvOp* op : P->convs) if (op->do_wgrad) { op->wacc = P->wacc_base ? P->wacc_base + off : nullptr; off += (op->wacc_elems() + 63) & ~size_t(63); }
   }

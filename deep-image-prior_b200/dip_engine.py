@@ -363,7 +363,13 @@ class FusedAdam:
 
 
 def run_iterations(plan, adam, z0, target, mask, sigma, seed, iters, lr, out=None, loss_hist=None):
-    """Closure-free device loop (dip_run_iterations): noise -> forward -> MSE -> backward -> Adam, `iters` times."""
+    """Closure-free device loop (dip_run_iterations): noise -> forward -> MSE -> backward -> Adam, `iters` times.
+    The device loop's Adam step uses torch's default betas and eps; an optimiser with others is refused, not stepped
+    with the defaults."""
+    if tuple(adam.betas) != (0.9, 0.999):
+        raise ValueError("dip-b200: run_iterations steps Adam with betas (0.9, 0.999); adam.betas is %r" % (adam.betas,))
+    if adam.eps != 1e-8:
+        raise ValueError("dip-b200: run_iterations steps Adam with eps 1e-8; adam.eps is %r" % (adam.eps,))
     with torch.cuda.device(plan.device):
         check(lib().dip_run_iterations(plan.h, adam.h, _ptr(z0), _ptr(target), _ptr(mask), float(sigma), int(seed),
                                        adam.step_count, int(iters), float(lr), _ptr(out), _ptr(loss_hist), _stream()))

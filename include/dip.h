@@ -134,7 +134,8 @@ int dip_adam_step(dip_adam* a, double lr, double beta1, double beta2, double eps
 /* ---- closure-free runner: `iters` iterations of  noise -> forward -> MSE -> backward -> Adam  entirely on the
  *      device (utils/common_utils.py:227-230 with the lean closure of denoising.ipynb c10).  m, v: Adam state
  *      (ntensors buffers).  Losses (device doubles, one per iteration) are written to loss_hist if non-NULL.
- *      step0 = number of Adam steps already taken. */
+ *      step0 = number of Adam steps already taken.
+ *      The runner's Adam step uses torch's defaults: betas (0.9, 0.999), eps 1e-8. */
 int dip_run_iterations(dip_plan* plan, dip_adam* adam, const void* z0, const void* target, const void* mask,
                        float sigma, uint64_t seed, int step0, int iters, double lr, void* out, double* loss_hist,
                        dip_stream_t stream);
