@@ -47,6 +47,11 @@ class SkipConfig:
     # in-net downsampling of the first down conv (models/common.py:101-113): 'stride' (stride-2 conv) or 'avg'
     # (stride-1 conv + nn.AvgPool2d(2, 2): restoration.ipynb c7:28-36 kate)
     downsample_mode = "stride"
+    # padding of every conv with k > 1 (models/common.py:114-120): 'reflection' is nn.ReflectionPad2d(k // 2), any other
+    # value Conv2d(padding=k // 2), i.e. zeros (models.skip's own default is pad='zero')
+    pad = "reflection"
+    # activation behind every BatchNorm but the concat's (models/common.py:76-92): a key of ACTIVATIONS
+    act_fun = "LeakyReLU"
 
     def nd(self, l):
         return self.channels[l] if isinstance(self.channels, (list, tuple)) else self.channels
@@ -130,7 +135,7 @@ def init_params(cfg, seed=None, dtype=torch.float32):
 # convs, 8 or more output channels -- reads its input, its weight and, in the backward pass, the incoming gradient
 # ROUNDED TO BF16 (round to nearest even), multiplies exactly and accumulates in fp32; biases, BatchNorm, activations,
 # up-sampling, the skinny skip convs, the head, the loss and Adam stay fp32.  `with operand_rounding('bf16'):` makes
-# _conv evaluate exactly that definition on the CPU (in whatever dtype the parameters have, fp64 included).
+# conv2d evaluate exactly that definition on the CPU (in whatever dtype the parameters have, fp64 included).
 _OPERAND_ROUND = None
 _MIN_TENSOR_CORE_WIDTH = 8   # the skinny skip convs (4 outputs) and the head (<= 4) run in fp32 on the CUDA cores
 
@@ -170,10 +175,10 @@ class _ConvBf16Operands(torch.autograd.Function):
         return dx, dw, dy.sum((0, 2, 3)), None
 
 
-def _conv(x, w, b, stride=1):
+def conv2d(x, w, b, stride=1, pad="reflection"):
     k = w.shape[-1]
-    if k > 1:
-        x = F.pad(x, (k // 2,) * 4, mode="reflect")  # nn.ReflectionPad2d, models/common.py:116-118
+    if k > 1:   # nn.ReflectionPad2d or Conv2d(padding=k // 2), models/common.py:114-120
+        x = F.pad(x, (k // 2,) * 4, mode="reflect" if pad == "reflection" else "constant")
     if _OPERAND_ROUND == "bf16" and w.shape[0] >= _MIN_TENSOR_CORE_WIDTH:
         return _ConvBf16Operands.apply(x, w, b, stride)
     return F.conv2d(x, w, b, stride=stride)
@@ -184,8 +189,19 @@ def _bn(x, g, b):
     return F.batch_norm(x, None, None, g, b, training=True, momentum=0.1, eps=1e-5)
 
 
-def _act(x):
-    return F.leaky_relu(x, 0.2)
+ACTIVATIONS = {"LeakyReLU": lambda x: F.leaky_relu(x, 0.2), "Swish": lambda x: x * torch.sigmoid(x), "ELU": F.elu,
+               "none": lambda x: x}   # act(): nn.LeakyReLU(0.2), Swish, nn.ELU(), nn.Sequential()
+
+
+def activation(x, kind="LeakyReLU"):
+    if kind not in ACTIVATIONS:
+        raise ValueError("act_fun must be one of %s, not %r" % (", ".join(ACTIVATIONS), kind))
+    return ACTIVATIONS[kind](x)
+
+
+# the earlier names (test_oracle.py calls _conv directly).  skip_forward calls conv2d and activation, so the padding and
+# the activation of a network come from its cfg alone, whatever a caller may have rebound these two names to.
+_conv, _act = conv2d, activation
 
 
 def skip_forward(params, z, cfg, tape=None):
@@ -196,21 +212,21 @@ def skip_forward(params, z, cfg, tape=None):
         pre = "L%d." % l
         s = None
         if cfg.ns(l) > 0:
-            s = _conv(x, P[pre + "skip.w"], P[pre + "skip.b"])
+            s = conv2d(x, P[pre + "skip.w"], P[pre + "skip.b"], pad=cfg.pad)
             if tape is not None:
                 tape[pre + "raw_s"] = s
-            s = _act(_bn(s, P[pre + "skip_bn.g"], P[pre + "skip_bn.b"]))
+            s = activation(_bn(s, P[pre + "skip_bn.g"], P[pre + "skip_bn.b"]), cfg.act_fun)
         if cfg.downsample_mode == "avg":
-            d = F.avg_pool2d(_conv(x, P[pre + "d1.w"], P[pre + "d1.b"], stride=1), 2, 2)
+            d = F.avg_pool2d(conv2d(x, P[pre + "d1.w"], P[pre + "d1.b"], stride=1, pad=cfg.pad), 2, 2)
         else:
-            d = _conv(x, P[pre + "d1.w"], P[pre + "d1.b"], stride=2)
+            d = conv2d(x, P[pre + "d1.w"], P[pre + "d1.b"], stride=2, pad=cfg.pad)
         if tape is not None:
             tape[pre + "raw_d1"] = d
-        d = _act(_bn(d, P[pre + "d1_bn.g"], P[pre + "d1_bn.b"]))
-        d = _conv(d, P[pre + "d2.w"], P[pre + "d2.b"])
+        d = activation(_bn(d, P[pre + "d1_bn.g"], P[pre + "d1_bn.b"]), cfg.act_fun)
+        d = conv2d(d, P[pre + "d2.w"], P[pre + "d2.b"], pad=cfg.pad)
         if tape is not None:
             tape[pre + "raw_d2"] = d
-        d = _act(_bn(d, P[pre + "d2_bn.g"], P[pre + "d2_bn.b"]))
+        d = activation(_bn(d, P[pre + "d2_bn.g"], P[pre + "d2_bn.b"]), cfg.act_fun)
         if l < cfg.num_scales - 1:
             d = rec(l + 1, d)
         mode = cfg.upsample_mode if isinstance(cfg.upsample_mode, str) else cfg.upsample_mode[l]   # per scale: skip.py:81
@@ -222,14 +238,14 @@ def skip_forward(params, z, cfg, tape=None):
         if tape is not None:
             tape[pre + "cat"] = c
         c = _bn(c, P[pre + "cat_bn.g"], P[pre + "cat_bn.b"])
-        u = _conv(c, P[pre + "up.w"], P[pre + "up.b"])
+        u = conv2d(c, P[pre + "up.w"], P[pre + "up.b"], pad=cfg.pad)
         if tape is not None:
             tape[pre + "raw_u"] = u
-        u = _act(_bn(u, P[pre + "up_bn.g"], P[pre + "up_bn.b"]))
-        v = _conv(u, P[pre + "c11.w"], P[pre + "c11.b"])
+        u = activation(_bn(u, P[pre + "up_bn.g"], P[pre + "up_bn.b"]), cfg.act_fun)
+        v = conv2d(u, P[pre + "c11.w"], P[pre + "c11.b"], pad=cfg.pad)
         if tape is not None:
             tape[pre + "raw_v"] = v
-        v = _act(_bn(v, P[pre + "c11_bn.g"], P[pre + "c11_bn.b"]))
+        v = activation(_bn(v, P[pre + "c11_bn.g"], P[pre + "c11_bn.b"]), cfg.act_fun)
         if tape is not None:
             tape[pre + "U"] = v
         return v

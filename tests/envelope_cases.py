@@ -1,7 +1,9 @@
-"""The envelope table: skip networks at the edges of what build_plan (csrc/engine.cu) and models.skip accept, shared by
-tests/test_envelope_cpu.py (reference anchor, composed stage references, routing) and tests/test_envelope_gpu.py (every
-stage of the engine against fp64 at its own inputs).  Each row is data; a planner change that widens or moves the
-accepted range adds a row here and both files pick it up.
+"""The networks of the stage tests, shared by the CPU tests (reference anchor, composed stage references, routing) and
+the GPU tests (every stage of the engine against fp64 at its own inputs): `cfg_of(kind, pad, act_fun)` builds the
+oracle's SkipConfig of a named network (NETS) or of a row of the envelope table.
+
+The envelope table: skip networks at the edges of what build_plan (csrc/engine.cu) and models.skip accept.  Each row is
+data; a planner change that widens or moves the accepted range adds a row here and the tests pick it up.
 
 Row fields: L (scales), in / out channels, per-scale down / up / skip widths, per-scale upsampling, downsample mode,
 H x W, need_sigmoid, and which extra GPU paths run on it: `zero_pad` (again with pad='zero'), `input_grad` (dz),
@@ -50,13 +52,40 @@ ROWS = [
 BY_ID = {r.id: r for r in ROWS}
 
 
-def cfg_of(row, pad="reflection"):
-    """the oracle's SkipConfig of a row (per-scale widths, channels_up set explicitly)"""
-    cfg = O.SkipConfig(in_channels=row.in_ch, out_channels=row.out_ch, num_scales=row.L, channels=list(row.down),
-                       skip_channels=list(row.skips), upsample_mode=list(row.modes), need_sigmoid=row.sigmoid)
-    cfg.channels_up = list(row.up)
-    cfg.downsample_mode = row.downsample
-    cfg.pad = pad
+MODES5 = ["bilinear", "nearest", "bilinear", "nearest", "nearest"]
+NETS = {
+    "cs4": lambda: O.SkipConfig(skip_channels=4, upsample_mode="bilinear"),
+    "cs128": lambda: O.SkipConfig(skip_channels=128, upsample_mode="nearest"),
+    "cs0": lambda: O.SkipConfig(skip_channels=0, upsample_mode="bilinear"),
+    "snail": lambda: O.SkipConfig(in_channels=3, channels=[8, 16, 32, 64, 128], skip_channels=[0, 0, 0, 4, 4]),
+    "kate": lambda: O.SkipConfig(in_channels=3, channels=[16, 32, 64, 128, 128], skip_channels=0),   # + 'avg'
+    "modes": lambda: O.SkipConfig(in_channels=3, skip_channels=4, upsample_mode=MODES5),
+    "ingrad": lambda: O.SkipConfig(skip_channels=4, out_channels=1, need_sigmoid=False),
+    # per-scale upsampling, logits as the output, one output channel (run with dL/d(input))
+    "modes_ingrad": lambda: O.SkipConfig(in_channels=3, out_channels=1, skip_channels=4, need_sigmoid=False,
+                                         upsample_mode=MODES5),
+    "per_scale128": lambda: O.SkipConfig(channels=[128] * 5, skip_channels=[4] * 5),
+    "avg128": lambda: O.SkipConfig(skip_channels=4),   # + 'avg'
+    # models.skip(32, 3)'s widths, skips and upsampling (its own default padding is 'zero': pass pad='zero')
+    "skipdefault": lambda: O.SkipConfig(upsample_mode="nearest", channels=[16, 32, 64, 128, 128], skip_channels=[4] * 5),
+}
+AVG = ("kate", "avg128")
+
+
+def cfg_of(kind, pad="reflection", act_fun="LeakyReLU"):
+    """the oracle's SkipConfig of a network of NETS or a row id of the envelope table (per-scale widths, channels_up set
+    explicitly), with the given padding and activation"""
+    if kind in BY_ID:
+        row = BY_ID[kind]
+        cfg = O.SkipConfig(in_channels=row.in_ch, out_channels=row.out_ch, num_scales=row.L, channels=list(row.down),
+                           skip_channels=list(row.skips), upsample_mode=list(row.modes), need_sigmoid=row.sigmoid)
+        cfg.channels_up = list(row.up)
+        cfg.downsample_mode = row.downsample
+    else:
+        cfg = NETS[kind]()
+        if kind in AVG:
+            cfg.downsample_mode = "avg"
+    cfg.pad, cfg.act_fun = pad, act_fun
     return cfg
 
 

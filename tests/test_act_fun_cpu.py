@@ -1,6 +1,7 @@
 """Activations other than LeakyReLU (models.skip's act_fun 'Swish', 'ELU', 'none') on the host side: the module tree
 against the live reference, the oracle against fixtures of the unmodified reference (tests/golden/make_act_fun.py), the
-act_refs stage references against the oracle's autograd, and the plan options of the C ABI (dip_plan_opts.act_fun).
+activations of the oracle and of the stage references, the stage references with each activation composed against the
+oracle's autograd (tests/test_stage_ref_cpu.py's check), and the plan options of the C ABI (dip_plan_opts.act_fun).
 No GPU needed."""
 import ctypes
 import os
@@ -9,62 +10,18 @@ import numpy as np
 import pytest
 import torch
 
-import act_refs as AR
 import models
 from oracle import dip_oracle as O
 from oracle import ref_harness
+import envelope_cases as E
 import stage_ref as SR
-from test_stage_ref_cpu import H, W, cfg_of
-from test_zero_pad_cpu import _desc
+from test_stage_ref_cpu import check_composed
+from test_zero_pad_cpu import _desc, oracle_cfg, setup
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 CASES = ["skipdefault64x96_swish", "denoise64x96_bilinear_elu", "inpaint64x96_nearest_masked_skip128_none",
          "restorekate64x96_avg_w16to128_swish"]
 KINDS = ["Swish", "ELU", "none"]
-
-
-def compose(cfg, params, z, target, input_grad):
-    """the stage references composed to the whole network (as tests/test_stage_ref_cpu.py), with cfg's padding and
-    activation"""
-    refs = SR.Refs()
-
-    def src(name):
-        if name.startswith("L") and name.endswith(".Pin") and name != "L0.Pin":   # a level's input = the level above's P_d2
-            name = "L%d.P_d2" % (int(name[1:-4]) - 1)
-        return refs[name]
-
-    AR.stage_forward(cfg, params, src, "fp64", refs, z=z)
-    out = refs["out"]
-    dout = 2.0 * (out - target[0]) / out.numel()
-    AR.stage_backward(cfg, params, src, "fp64", refs, dout, input_grad=input_grad)
-    return refs
-
-
-def oracle_cfg(g):
-    chans, skips = [int(x) for x in g["chans"]], [int(x) for x in g["skips"]]
-    modes = [str(m) for m in g["modes"]]
-    if set(chans) == {128} and len(set(skips)) == 1:
-        cfg = O.SkipConfig(in_channels=int(g["in_depth"]), out_channels=int(g["out_ch"]), upsample_mode=modes, skip_channels=skips[0])
-    else:
-        cfg = O.SkipConfig(in_channels=int(g["in_depth"]), out_channels=int(g["out_ch"]), upsample_mode=modes, channels=chans,
-                           skip_channels=skips)
-    cfg.downsample_mode = str(g["downsample_mode"])
-    cfg.pad = str(g["pad"])
-    cfg.act_fun = str(g["act_fun"])
-    return cfg
-
-
-def setup(g, dtype):
-    """the fixture's inputs, drawn as tests/golden/make_act_fun.py draws them"""
-    cfg = oracle_cfg(g)
-    H_, W_ = int(g["H"]), int(g["W"])
-    gen = torch.Generator().manual_seed(2)
-    z0 = torch.rand(1, cfg.in_channels, H_, W_, generator=gen).to(dtype)
-    target = torch.rand(1, cfg.out_channels, H_, W_, generator=gen).to(dtype)
-    mask = (torch.rand(1, 1, H_, W_, generator=gen) > 0.5).to(dtype) if bool(g["masked"]) else None
-    gn = torch.Generator().manual_seed(123)
-    noises = [torch.randn(z0.shape, generator=gn).to(dtype) for _ in range(int(g["iters"]))]
-    return cfg, z0, target, mask, noises
 
 
 def build_net(case, g):
@@ -126,9 +83,8 @@ def test_tree_equals_live_reference(act_fun):
     finally:
         models.allow_torch_execution(False)
     assert torch.allclose(out, rout, atol=1e-6)
-    cfg = O.SkipConfig(upsample_mode="nearest", channels=[16, 32, 64, 128, 128], skip_channels=[4] * 5)
-    cfg.act_fun = act_fun
-    assert torch.allclose(AR.skip_forward(O.init_params(cfg, seed=11), z, cfg).detach(), rout, atol=1e-6)
+    cfg = E.cfg_of("skipdefault", act_fun=act_fun)
+    assert torch.allclose(O.skip_forward(O.init_params(cfg, seed=11), z, cfg).detach(), rout, atol=1e-6)
 
 
 def test_get_net_forwards_act_fun():
@@ -160,7 +116,7 @@ def test_oracle_matches_reference_golden_fp64(case):
         if i == 0:
             rec["out0"], rec["grads0"] = out, [x.clone() for x in grads]
 
-    losses, _ = AR.run(cfg, params, z0, target, noises, float(g["sigma"]), float(g["lr"]), mask=mask, record=record)
+    losses, _ = O.run(cfg, params, z0, target, noises, float(g["sigma"]), float(g["lr"]), mask=mask, record=record)
     assert np.allclose(rec["out0"].numpy(), g["out0"], atol=1e-10)
     assert np.allclose(losses, g["losses"], rtol=1e-10)
     gn = np.array([x.double().norm().item() for x in rec["grads0"]])
@@ -177,12 +133,12 @@ def test_act_oracle_differs_from_leaky_relu(case):
     cfg, z0, _, _, noises = setup(g, torch.float64)
     params = O.init_params(cfg, seed=0, dtype=torch.float64)
     z = z0 + noises[0] * float(g["sigma"])
-    assert np.abs(AR.skip_forward(params, z, cfg).detach().numpy() - g["out0"]).max() < 1e-10
+    assert np.abs(O.skip_forward(params, z, cfg).detach().numpy() - g["out0"]).max() < 1e-10
     cfg.act_fun = "LeakyReLU"
-    assert np.abs(AR.skip_forward(params, z, cfg).detach().numpy() - g["out0"]).max() > 1e-4
+    assert np.abs(O.skip_forward(params, z, cfg).detach().numpy() - g["out0"]).max() > 1e-4
 
 
-# ------------------------------------------------------------------------------------------------ stage references
+# ------------------------------------------------------------------------------------------------ activations
 STAGE_CASES = [(k, kind, pad) for kind in KINDS for k, pad in
                (("cs4", "reflection"), ("cs4", "zero"), ("cs128", "reflection"), ("skipdefault", "zero"))] + \
               [("cs0", "Swish", "zero"), ("snail", "ELU", "reflection"), ("kate", "none", "zero"),
@@ -191,59 +147,34 @@ STAGE_CASES = [(k, kind, pad) for kind in KINDS for k, pad in
 
 @pytest.mark.parametrize("net,kind,pad", STAGE_CASES)
 def test_composed_act_stages_reproduce_the_oracle(net, kind, pad):
-    """tests/stage_ref.py under act_refs (the activation and its derivative in fp64), composed stage by stage, against
-    the oracle's network with the same activation and its autograd gradients (as tests/test_stage_ref_cpu.py)"""
-    if net == "skipdefault":
-        cfg = O.SkipConfig(upsample_mode="nearest", channels=[16, 32, 64, 128, 128], skip_channels=[4] * 5)
-    else:
-        cfg = cfg_of(net)
-    cfg.pad, cfg.act_fun = pad, kind
-    input_grad = net == "modes_ingrad"
-    params = SR.random_affine(cfg, O.init_params(cfg, seed=0, dtype=torch.float64), seed=7)
-    g = torch.Generator().manual_seed(3)
-    z = torch.rand(1, cfg.in_channels, H, W, generator=g, dtype=torch.float64)
-    target = torch.rand(1, cfg.out_channels, H, W, generator=g, dtype=torch.float64)
-    refs = compose(cfg, params, z, target, input_grad)
-    assert refs.excl and all(frac == 0 for frac, _ in refs.excl.values())
-    assert all(e is None or not e.any() for _, _, e in refs.d.values())
-
-    p = [x.detach().clone().requires_grad_(True) for x in params]
-    zz = z.clone().requires_grad_(input_grad)
-    out = AR.skip_forward(p, zz, cfg)
-    assert (refs["out"] - out.detach()[0]).abs().max().item() < 1e-12
-    grads = torch.autograd.grad(O.mse_loss(out, target), p + ([zz] if input_grad else []))
-    names = [n for n, _ in O.param_layout(cfg)] + (["dz"] if input_grad else [])
-    gmax = max(gr.abs().max().item() for gr in grads)
-    for name, gr in zip(names, grads):
-        got = refs[name if name == "dz" else "grad:" + name].reshape(gr.shape)
-        err = (got - gr).abs().max().item()
-        assert err <= max(1e-10 * gr.abs().max().item(), 1e-13 * gmax), (name, err, gr.abs().max().item())
+    """tests/stage_ref.py with the activation and its derivative in fp64, composed stage by stage, against the oracle's
+    network with the same activation and its autograd gradients (tests/test_stage_ref_cpu.py's check, which also finds
+    no excluded element)"""
+    check_composed(E.cfg_of(net, pad, kind), 64, 96, net == "modes_ingrad")
 
 
-def test_activation_swaps_only_for_other_kinds():
-    """LeakyReLU configurations (and configurations without act_fun) keep the references' own functions; the other
-    kinds swap them only inside the context"""
-    saved = (O._act, SR.Bn)
-    cfg = O.SkipConfig()
-    with AR.activation(cfg):
-        assert (O._act, SR.Bn) == saved
-    cfg.act_fun = "LeakyReLU"
-    with AR.activation(cfg):
-        assert (O._act, SR.Bn) == saved
+def test_activation_values_and_derivatives():
+    """the oracle's activations against their closed forms (an unknown kind is refused), the derivative stage_ref applies
+    against autograd of them, and the concat BatchNorm applies no activation"""
     y = torch.linspace(-30, 30, 601, dtype=torch.float64).reshape(-1, 1)
     expect = {"Swish": y * torch.sigmoid(y), "ELU": torch.where(y > 0, y, torch.expm1(y)), "none": y}
     for kind in KINDS:
-        cfg.act_fun = kind
-        with AR.activation(cfg):
-            assert O._act is not saved[0] and SR.Bn is not saved[1] and issubclass(SR.Bn, saved[1])
-            assert torch.allclose(O._act(y), expect[kind], rtol=1e-14, atol=1e-300)
-            # the derivative the Bn subclass applies, against autograd of the oracle's activation
-            yy = y.clone().requires_grad_(True)
-            d_auto = torch.autograd.grad(O._act(yy).sum(), yy)[0]
-            assert torch.allclose(AR.GRAD[kind](y), d_auto, rtol=1e-12, atol=1e-300)
-        assert (O._act, SR.Bn) == saved
-    # the concat BatchNorm keeps stage_ref's own base class
-    assert SR.CatBn.__bases__ == (saved[1],)
+        assert torch.allclose(O._act(y, kind), expect[kind], rtol=1e-14, atol=1e-300)
+        yy = y.clone().requires_grad_(True)
+        d_auto = torch.autograd.grad(O._act(yy, kind).sum(), yy)[0]
+        assert torch.allclose(SR.GRAD[kind](y), d_auto, rtol=1e-12, atol=1e-300)
+    for bad in ("relu", "leakyrelu", None):
+        with pytest.raises(ValueError, match="act_fun"):
+            O._act(y, bad)
+    raw = torch.randn(6, 4, 8, dtype=torch.float64)
+    g, b = torch.rand(8, dtype=torch.float64) + 0.5, torch.rand(8, dtype=torch.float64) - 0.5
+    plain = SR.Bn(raw, g, b).out(act=False)
+    gout = torch.randn(6, 4, 8, dtype=torch.float64)
+    for kind in KINDS:   # (CatBn runs out / backward with act=False only)
+        bn = SR.Bn(raw, g, b, kind)
+        assert torch.equal(bn.out(act=False), plain) and torch.equal(bn.out(), SR.FWD[kind](plain))
+        res = bn.backward(gout, act=False)
+        assert torch.equal(res["dx"], SR.Bn(raw, g, b).backward(gout, act=False)["dx"]) and not res["excl"].any()
 
 
 # ------------------------------------------------------------------------------------------------ C ABI

@@ -1,7 +1,7 @@
-"""Activations other than LeakyReLU on the engine (H100): every stage of one forward + backward against its fp64
-reference at the engine's own inputs (tests/stage_ref.py under act_refs, the tolerances of tests/test_stages_gpu.py,
-every registered buffer NaN-filled first, no element excluded), the device runner, the notebook-facing API against
-fixtures of the unmodified reference (tests/golden/make_act_fun.py), and LeakyReLU given explicitly = NULL options."""
+"""Activations other than LeakyReLU on the engine (H100): every stage of the networks with each activation against the
+fp64 references, through the harness of tests/test_stages_gpu.py (which also checks that no element is excluded from
+the backward checks), the notebook-facing API against fixtures of the unmodified reference (tests/golden/make_act_fun.py),
+and LeakyReLU given explicitly = NULL options."""
 import ctypes
 import os
 
@@ -9,70 +9,14 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import dip_oracle as O
-import act_refs as AR
-import stage_ref as SR
+import envelope_cases as E
 import test_stages_gpu as TS
-from test_act_fun_cpu import CASES as GOLD_CASES, GOLD, build_net, setup
+from test_act_fun_cpu import CASES as GOLD_CASES, GOLD, build_net
+from test_zero_pad_cpu import setup
 
 pytestmark = pytest.mark.gpu
 MODES = ["fp32", "tf32", "bf16"]
 KINDS = ["Swish", "ELU", "none"]
-
-
-def cfg_of(kind, act_fun):
-    if kind == "skipdefault":   # models.skip(32, 3): widths [16, 32, 64, 128, 128], skips 4, nearest, pad='zero'
-        cfg = O.SkipConfig(upsample_mode="nearest", channels=[16, 32, 64, 128, 128], skip_channels=[4] * 5)
-        cfg.pad = "zero"
-    else:
-        cfg = TS.cfg_of(kind)
-    cfg.act_fun = act_fun
-    return cfg
-
-
-def make_plan(cfg, H, W, mode, input_grad=False):
-    import dip_engine as de
-    prec = {"fp32": de.PRECISION_FP32, "tf32": de.PRECISION_TF32, "bf16": de.PRECISION_BF16}[mode]
-    bil = cfg.upsample_mode == "bilinear" if isinstance(cfg.upsample_mode, str) else [m == "bilinear" for m in cfg.upsample_mode]
-    L = cfg.num_scales
-    per_scale = isinstance(cfg.channels, (list, tuple)) or isinstance(cfg.skip_channels, (list, tuple))
-    ch = [cfg.nd(l) for l in range(L)] if per_scale else cfg.channels
-    sk = [cfg.ns(l) for l in range(L)] if per_scale else cfg.skip_channels
-    return de.Plan(cfg.in_channels, cfg.out_channels, L, ch, sk, bil, H, W, precision=prec, need_sigmoid=cfg.need_sigmoid,
-                   input_grad=input_grad, downsample_mode=cfg.downsample_mode, pad=getattr(cfg, "pad", "reflection"),
-                   act=AR.act_of(cfg))
-
-
-def check_no_exclusion(refs):
-    """no activation here has a jump in its derivative: not one element may be excluded from the backward checks"""
-    assert refs.excl, "no BN(+act) backward was checked"
-    shares = {name: frac for name, (frac, _) in refs.excl.items()}
-    assert all(frac == 0.0 for frac in shares.values()), shares
-    assert all(e is None or not e.any() for _, _, e in refs.d.values())
-
-
-def run_direct(cfg, H, W, mode, input_grad=False, seed=0):
-    params = TS.params_for(cfg, seed)
-    g = torch.Generator().manual_seed(seed + 1)
-    z = torch.rand(1, cfg.in_channels, H, W, generator=g).cuda()
-    target = torch.rand(1, cfg.out_channels, H, W, generator=g).cuda()
-    plan = make_plan(cfg, H, W, mode, input_grad)
-    dparams = [p.cuda().contiguous() for p in params]
-    dgrads = [torch.zeros_like(p) for p in dparams]
-    plan.bind(dparams, dgrads)
-    TS.fill_nan(plan, cfg.num_scales)
-    out = plan.forward(z)
-    dout = (2.0 * (out - target) / out.numel()).contiguous()
-    plan.backward(dout)
-    dz = plan.input_grad() if input_grad else None
-    torch.cuda.synchronize()
-    refs = SR.Refs()
-    src = plan.buffer if mode != "bf16" else (lambda n: TS.buffer_view(plan, n) if n.endswith("16") else plan.buffer(n))
-    AR.stage_forward(cfg, dparams, lambda n: out[0] if n == "out" else src(n), mode, refs, z=z)
-    AR.stage_backward(cfg, dparams, lambda n: out[0] if n == "out" else src(n), mode, refs, dout[0], input_grad=input_grad)
-    check_no_exclusion(refs)
-    TS.check("%s %s %dx%d" % (cfg.act_fun, TS.cfg_tag(cfg), H, W), cfg, mode, plan, refs, dgrads, out, dz)
-
 
 NETS = {"cs4": (64, 96, False), "skipdefault": (64, 96, False), "cs128": (96, 64, False), "cs0": (64, 96, False),
         "kate": (96, 64, False), "snail": (64, 96, False), "ingrad": (64, 96, True)}
@@ -83,56 +27,14 @@ ONE_MODE = {"cs128": ("tf32", "bf16", "fp32"), "cs0": ("bf16", "fp32", "tf32"), 
 DIRECT = [(net, act, mode) for net in ("cs4", "skipdefault") for act in KINDS for mode in MODES] + \
          [(net, act, modes[i]) for net, modes in ONE_MODE.items() for i, act in enumerate(KINDS)]
 
+PAD = {"skipdefault": "zero"}   # the skip() default network as models.skip builds it; the others pad by reflection
+
 
 @pytest.mark.parametrize("net,act,mode", DIRECT, ids=["%s_%s_%s" % c for c in DIRECT])
 def test_every_stage_act(net, act, mode):
     H, W, input_grad = NETS[net]
-    run_direct(cfg_of(net, act), H, W, mode, input_grad)
+    TS.run_direct(E.cfg_of(net, PAD.get(net, "reflection"), act), H, W, mode, input_grad)
     TS.print_table()
-
-
-def run_runner(cfg, H, W, mode, task):
-    """one iteration of the device runner at lr = 0 (Adam leaves the parameters bitwise unchanged), every stage checked"""
-    import dip_engine as de
-    params = TS.params_for(cfg, 3)
-    g = torch.Generator().manual_seed(5)
-    z0 = torch.rand(1, cfg.in_channels, H, W, generator=g).cuda()
-    plan = make_plan(cfg, H, W, mode)
-    mask = down = None
-    if task == "sr":
-        kern = O.down_kernel(4, "lanczos2", 0.5)
-        down = (torch.from_numpy(kern).double(), 4, O.down_pad(kern.shape[0], 4))
-        plan.set_downsampler(torch.from_numpy(kern).float(), 4, down[2])
-        th, tw = de.down_out_size(H, kern.shape[0], 4, down[2]), de.down_out_size(W, kern.shape[0], 4, down[2])
-    else:
-        th, tw = H, W
-    target = torch.rand(1, cfg.out_channels, th, tw, generator=g).cuda()
-    if task == "inpaint":
-        mask = (torch.rand(1, 1, H, W, generator=g) > 0.3).float().cuda()
-    dparams = [p.cuda().contiguous() for p in params]
-    dgrads = [torch.zeros_like(p) for p in dparams]
-    plan.bind(dparams, dgrads)
-    for p, gb in zip(dparams, dgrads):
-        p.grad = gb
-    adam = de.FusedAdam(dparams, lr=0.0)
-    adam._bind(dgrads)
-    before = [p.clone() for p in dparams]
-    TS.fill_nan(plan, cfg.num_scales)
-    out = torch.empty(1, cfg.out_channels, H, W, device="cuda")
-    de.run_iterations(plan, adam, z0, target, mask, 1. / 30, 7, 1, 0.0, out=out)
-    torch.cuda.synchronize()
-    assert all(torch.equal(a, b) for a, b in zip(before, dparams))
-    o = out.double().cpu().requires_grad_(True)
-    lo = o if down is None else O.downsample(o, *down)
-    loss = O.mse_loss(lo, target.double().cpu(), None if mask is None else mask.double().cpu())
-    dout = torch.autograd.grad(loss, o)[0].cuda()
-    src = plan.buffer if mode != "bf16" else (lambda n: TS.buffer_view(plan, n) if n.endswith("16") else plan.buffer(n))
-    rd = lambda n: out[0] if n == "out" else src(n)   # noqa: E731
-    refs = SR.Refs()
-    AR.stage_forward(cfg, dparams, rd, mode, refs)
-    AR.stage_backward(cfg, dparams, rd, mode, refs, dout[0])
-    check_no_exclusion(refs)
-    TS.check("%s runner %s %s %dx%d" % (cfg.act_fun, task, TS.cfg_tag(cfg), H, W), cfg, mode, plan, refs, dgrads, out)
 
 
 @pytest.mark.parametrize("task,act,kind,H,W,mode", [("denoise", "Swish", "cs4", 128, 128, "tf32"),
@@ -140,7 +42,7 @@ def run_runner(cfg, H, W, mode, task):
                                                      ("sr", "none", "cs4", 256, 256, "tf32"),
                                                      ("sr", "none", "cs4", 256, 256, "bf16")])
 def test_every_stage_runner_act(task, act, kind, H, W, mode):
-    run_runner(cfg_of(kind, act), H, W, mode, task)
+    TS.run_runner(E.cfg_of(kind, PAD.get(kind, "reflection"), act), H, W, mode, task)
     TS.print_table()
 
 
@@ -231,7 +133,7 @@ def test_explicit_leaky_relu_equals_null_opts(mode):
     """act_fun = DIP_ACT_LEAKY_RELU given explicitly computes bitwise what a plan with NULL options computes (and Swish
     does not)"""
     import dip_engine as de
-    cfg = TS.cfg_of("cs4")
+    cfg = E.cfg_of("cs4")
     H, W = 64, 96
     params = [p.cuda().contiguous() for p in TS.params_for(cfg, 0)]
     g = torch.Generator().manual_seed(1)
@@ -240,7 +142,7 @@ def test_explicit_leaky_relu_equals_null_opts(mode):
     results = {}
     for name in ("explicit", "null", "swish"):
         cfg.act_fun = "Swish" if name == "swish" else "LeakyReLU"
-        plan = make_plan(cfg, H, W, mode)
+        plan = TS.make_plan(cfg, H, W, mode)
         if name == "explicit":
             assert (plan.opts.pad_mode, plan.opts.act_fun) == (de.PAD_REFLECTION, de.ACT_LEAKY_RELU)
         if name == "null":

@@ -9,9 +9,7 @@ import models
 from oracle import dip_oracle as O
 from oracle import ref_harness
 import envelope_cases as E
-import pad_refs as PR
-import stage_ref as SR
-from test_zero_pad_cpu import compose
+from test_stage_ref_cpu import check_composed
 
 CASES = [(r.id, pad) for r in E.ROWS for pad in E.pads_of(r)]
 IDS = ["%s_%s" % c for c in CASES]
@@ -23,7 +21,7 @@ def test_reference_anchor(rid, pad):
     """the reference's network at the row's arguments: the oracle's init draws are its parameters bit for bit, and the
     oracle's forward is its forward in fp64"""
     row = E.BY_ID[rid]
-    cfg = E.cfg_of(row, pad)
+    cfg = E.cfg_of(rid, pad)
     with ref_harness.reference_modules() as ref:
         torch.manual_seed(0)
         rnet = ref.models.skip(**E.skip_kwargs(row, pad))
@@ -35,39 +33,16 @@ def test_reference_anchor(rid, pad):
     assert [tuple(p.shape) for p in rparams] == [tuple(p.shape) for p in params]
     for (name, _), a, b in zip(O.param_layout(cfg), rparams, params):
         assert torch.equal(a, b.detach()), name
-    out = PR.skip_forward([p.detach().double() for p in params], z, cfg).detach()
+    out = O.skip_forward([p.detach().double() for p in params], z, cfg).detach()
     assert out.shape == rout.shape and (out - rout).abs().max().item() <= 1e-12
 
 
 @pytest.mark.parametrize("rid,pad", CASES, ids=IDS)
 def test_composed_stages_reproduce_the_oracle(rid, pad):
-    """tests/stage_ref.py composed stage by stage against the oracle's output and autograd gradients, dz included, at the
-    bounds of tests/test_stage_ref_cpu.py"""
+    """tests/stage_ref.py composed stage by stage against the oracle's output and autograd gradients, dz included
+    (tests/test_stage_ref_cpu.py's check)"""
     row = E.BY_ID[rid]
-    cfg = E.cfg_of(row, pad)
-    params = SR.random_affine(cfg, O.init_params(cfg, seed=0, dtype=torch.float64), seed=7)
-    g = torch.Generator().manual_seed(3)
-    z = torch.rand(1, cfg.in_channels, row.H, row.W, generator=g, dtype=torch.float64)
-    target = torch.rand(1, cfg.out_channels, row.H, row.W, generator=g, dtype=torch.float64)
-    refs = compose(cfg, params, z, target, True)
-    pin = refs["L0.Pin"]   # the stored depth's channels after the real ones are zeros
-    assert pin.shape[-1] == SR.stored_depth(cfg, 0) and pin[..., cfg.in_channels:].abs().sum().item() == 0
-
-    p = [x.detach().clone().requires_grad_(True) for x in params]
-    zz = z.clone().requires_grad_(True)
-    out = PR.skip_forward(p, zz, cfg)
-    assert (refs["out"] - out.detach()[0]).abs().max().item() < 1e-12
-    grads = torch.autograd.grad(O.mse_loss(out, target), p + [zz])
-    names = [n for n, _ in O.param_layout(cfg)] + ["dz"]
-    gmax = max(gr.abs().max().item() for gr in grads)
-    for name, gr in zip(names, grads):
-        got = refs[name if name == "dz" else "grad:" + name].reshape(gr.shape)
-        err = (got - gr).abs().max().item()
-        assert err <= max(1e-10 * gr.abs().max().item(), 1e-13 * gmax), (name, err, gr.abs().max().item())
-        if SR.is_dead_bias(name):
-            assert got.abs().max().item() == 0, name
-        if name.endswith(".w") and name != "head.w":
-            assert "grad:" + name in refs.conv, name
+    check_composed(E.cfg_of(rid, pad), row.H, row.W, True)
 
 
 @pytest.mark.parametrize("rid,pad", CASES, ids=IDS)
@@ -87,7 +62,7 @@ def test_models_skip_routes_the_row_to_the_engine(rid, pad):
     assert per(spec["skip_channels"]) == row.skips
     assert per(spec["bilinear"]) == [m == "bilinear" for m in row.modes]
     assert spec["pad"] == pad and spec["downsample_mode"] == row.downsample and spec["need_sigmoid"] == row.sigmoid
-    cfg = E.cfg_of(row, pad)
+    cfg = E.cfg_of(rid, pad)
     for (name, shape), a, b in zip(O.param_layout(cfg), net.parameters(), O.init_params(cfg, seed=0)):
         assert tuple(a.shape) == tuple(shape) and torch.equal(a.detach(), b.detach()), name
     assert len(list(net.parameters())) == len(O.param_layout(cfg))

@@ -14,10 +14,9 @@ every configuration makes four calls on one plan and one FusedAdam at lr = 0.01,
 Before each call the level buffers, every gradient buffer and the weight-gradient partials ("wacc", tensor-core modes)
 are filled with NaN, and p, m, v are copied.  After each call:
 
-* stages: every stage and every parameter gradient through TS.check (the stage references of tests/stage_ref.py under
-  tests/act_refs.py, which also carries the zero padding of tests/pad_refs.py; the tolerances of tests/test_stages_gpu.py)
-  at the parameters the last iteration's forward used: the copy taken before a one-iteration call, and for C the
-  parameters reconstructed from the state the call left (below).  Stale weight packs fail the convolutions by orders of
+* stages: every stage and every parameter gradient through TS.check (the stage references of tests/stage_ref.py at the
+  configuration's padding and activation; the tolerances of tests/test_stages_gpu.py) at the parameters the last
+  iteration's forward used: the copy taken before a one-iteration call, and for C the parameters reconstructed from the state the call left (below).  Stale weight packs fail the convolutions by orders of
   magnitude; a gradient that accumulates or is not written fails its 'grad:' entry or comes out NaN;
 * Adam (one-iteration calls): from the copied p, m, v, the gradients the call left and step = steps before + 1,
       m* = b1 m + (1 - b1) g,  v* = b2 v + (1 - b2) g^2          (fp64)
@@ -29,9 +28,9 @@ are filled with NaN, and p, m, v are copied.  After each call:
   exactly;
 * C, the last of three iterations: the parameters its forward used are p_C + U(m_C, v_C, step 5), reconstructed in fp64
   from the engine's state after the call.  With U_k the kernel's own update, p_C = fl(x - U_k) and |U_k - U| <= 7u |U|,
-  so the reconstruction is within delta = 2u |p_C| + 8u |U| of the true x.  That uncertainty is added to the tolerance of
-  every convolution that multiplies a parameter: conv(|input|, delta_w) + delta_b (conv_transpose for the input
-  gradients); in bf16 mode the tensor-core convolutions multiply bf16(x), so their weight uncertainty is
+  so the reconstruction is within delta = 2u |p_C| + 8u |U| of the true x.  stage_ref adds that uncertainty to the
+  tolerance of every convolution that multiplies a parameter: conv(|input|, delta_w) + delta_b (conv_transpose for the
+  input gradients); in bf16 mode the tensor-core convolutions multiply bf16(x), so their weight uncertainty is
   bf16(x + delta) - bf16(x - delta), one bf16 ulp where a rounding boundary lies within delta of x, 0 elsewhere.  A wrong
   step number, or packs of the weights of an earlier iteration, reconstructs parameters that are off by a whole Adam
   step and the convolutions fail;
@@ -60,20 +59,15 @@ import os
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 from oracle import dip_oracle as O
-import act_refs as AR
 import envelope_cases as E
-import pad_refs as PR
 import stage_ref as SR
-import test_act_fun_gpu as AG
 import test_stages_gpu as TS
-from test_envelope_gpu import engine_src
 
 pytestmark = pytest.mark.gpu
 U = 2.0 ** -24
-LR, SIGMA, SEED = 0.01, 1. / 30, 7
+LR, SIGMA, SEED = 0.01, TS.SIGMA, TS.SEED
 BETAS, EPS = (0.9, 0.999), 1e-8
 CALLS = [("A", 1, 0), ("B", 1, 1), ("C", 3, 2), ("D", 1, 5)]   # (call, iterations, Adam steps taken before)
 HIST = 5                       # loss_hist slots; every call leaves the ones after its iterations at -1
@@ -84,21 +78,21 @@ LOSS = {}                      # mode -> worst |slot - fp64 MSE| / bound
 # (id, task, SkipConfig, H, W, precision mode): the comment names what only that configuration reaches
 CONFIGS = [
     # the flagship schedule: deferred weight gradients and side streams
-    ("denoise_cs4_tf32", "denoise", lambda: TS.cfg_of("cs4"), 128, 128, "tf32"),
+    ("denoise_cs4_tf32", "denoise", lambda: E.cfg_of("cs4"), 128, 128, "tf32"),
     # bf16 weight twins repacked every iteration
-    ("denoise_cs4_bf16", "denoise", lambda: TS.cfg_of("cs4"), 128, 128, "bf16"),
+    ("denoise_cs4_bf16", "denoise", lambda: E.cfg_of("cs4"), 128, 128, "bf16"),
     # the SIMT convolutions and k_wgrad_reduce
-    ("denoise_cs4_fp32", "denoise", lambda: TS.cfg_of("cs4"), 64, 96, "fp32"),
+    ("denoise_cs4_fp32", "denoise", lambda: E.cfg_of("cs4"), 64, 96, "fp32"),
     # the two-part up-conv weight gradient (up_a / up_b) into one tensor; the masked loss
-    ("inpaint_cs128_tf32", "inpaint", lambda: TS.cfg_of("cs128"), 128, 192, "tf32"),
+    ("inpaint_cs128_tf32", "inpaint", lambda: E.cfg_of("cs128"), 128, 192, "tf32"),
     # ds_y / ds_dy and the loss on the low-resolution output
-    ("sr_cs4_bf16", "sr", lambda: TS.cfg_of("cs4"), 256, 256, "bf16"),
+    ("sr_cs4_bf16", "sr", lambda: E.cfg_of("cs4"), 256, 256, "bf16"),
     # skinny 1x1 convolutions with fp64-atomic weight gradients
-    ("denoise_snail_tf32", "denoise", lambda: TS.cfg_of("snail"), 64, 96, "tf32"),
+    ("denoise_snail_tf32", "denoise", lambda: E.cfg_of("snail"), 64, 96, "tf32"),
     # W % 4 = 2: the separate k_noise -> zbuf path
-    ("denoise_L1_tf32", "denoise", lambda: E.cfg_of(E.BY_ID["L1"]), 10, 14, "tf32"),
+    ("denoise_L1_tf32", "denoise", lambda: E.cfg_of("L1"), 10, 14, "tf32"),
     # zero padding (k_noise_pad<true>) and the templated BatchNorm kernels of Swish over several iterations
-    ("denoise_skipdefault_swish_tf32", "denoise", lambda: AG.cfg_of("skipdefault", "Swish"), 64, 96, "tf32"),
+    ("denoise_skipdefault_swish_tf32", "denoise", lambda: E.cfg_of("skipdefault", "zero", "Swish"), 64, 96, "tf32"),
 ]
 BY_ID = {c[0]: c[1:] for c in CONFIGS}
 
@@ -186,77 +180,14 @@ def check_adam(tag, before, g, after, lr, betas, eps, step):
     assert not failures, "[Adam %s, step %d]\n  " % (tag, step) + "\n  ".join(failures)
 
 
-# ------------------------------------------------------------------------------------------------ uncertain parameters
-@contextlib.contextmanager
-def uncertain_params(cfg, delta):
-    """stage_ref's convolution tolerances plus the propagated uncertainty of reconstructed parameters (module docstring):
-    delta[i] bounds |reconstructed - true| of parameter i (param_layout order)"""
-    dw = {n: d.double() for (n, _), d in zip(O.param_layout(cfg), delta)}
-    params0, w0, conv0, dgrad0 = SR._params, SR._Reader.w, SR.conv, SR.conv_dgrad
-
-    def params_(cfg_, ps):
-        P = params0(cfg_, ps)
-        for n, t in P.items():
-            t.unc = dw[n]
-        return P
-
-    def w_(self, name):
-        t = w0(self, name)
-        if self.mode == "bf16":   # the tensor-core kernels multiply bf16(x)
-            x, d = self.P[name], dw[name]
-            t.unc = SR.bf16(x + d) - SR.bf16(x - d)
-        return t
-
-    def conv_(x, w, b, stride, mode):
-        y, tol = conv0(x, w, b, stride, mode)
-        e = F.conv2d(SR.nchw(x.double().abs()), w.unc, None if b is None else b.unc, stride=stride)
-        return y, tol + SR.hwc(e)
-
-    def dgrad_(dy, w, stride, mode):
-        g, tol = dgrad0(dy, w, stride, mode)
-        e = F.conv_transpose2d(SR.nchw(dy.double().abs()), w.unc, stride=stride)
-        if stride == 2:
-            e = F.pad(e, (0, 1, 0, 1))
-        return g, tol + SR.hwc(e)
-
-    SR._params, SR._Reader.w, SR.conv, SR.conv_dgrad = params_, w_, conv_, dgrad_
-    try:
-        yield
-    finally:
-        SR._params, SR._Reader.w, SR.conv, SR.conv_dgrad = params0, w0, conv0, dgrad0
-
-
 # ------------------------------------------------------------------------------------------------ the runner
-class Runner:
-    """one plan, one FusedAdam and the inputs of a runner configuration (the setup of test_stages_gpu.run_runner)"""
+class Runner(TS.Runner):
+    """the plan, FusedAdam and inputs of a runner configuration (test_stages_gpu.Runner) at lr = LR"""
 
     def __init__(self, cid):
-        import dip_engine as de
         task, make_cfg, H, W, mode = BY_ID[cid]
-        self.cid, self.task, self.mode = cid, task, mode
-        self.cfg = cfg = make_cfg()
-        g = torch.Generator().manual_seed(5)
-        self.z0 = torch.rand(1, cfg.in_channels, H, W, generator=g).cuda()
-        self.plan = AG.make_plan(cfg, H, W, mode)
-        self.mask = self.down = None
-        if task == "sr":
-            kern = O.down_kernel(4, "lanczos2", 0.5)
-            self.down = (torch.from_numpy(kern).double(), 4, O.down_pad(kern.shape[0], 4))
-            self.plan.set_downsampler(torch.from_numpy(kern).float(), 4, self.down[2])
-            th, tw = de.down_out_size(H, kern.shape[0], 4, self.down[2]), de.down_out_size(W, kern.shape[0], 4, self.down[2])
-        else:
-            th, tw = H, W
-        self.target = torch.rand(1, cfg.out_channels, th, tw, generator=g).cuda()
-        if task == "inpaint":
-            self.mask = (torch.rand(1, 1, H, W, generator=g) > 0.3).float().cuda()
-        self.params = [p.cuda().contiguous() for p in TS.params_for(cfg, 3)]
-        self.grads = [torch.zeros_like(p) for p in self.params]
-        self.plan.bind(self.params, self.grads)
-        for p, gb in zip(self.params, self.grads):
-            p.grad = gb
-        self.adam = de.FusedAdam(self.params, lr=LR)
-        self.adam._bind(self.grads)
-        self.out = torch.empty(1, cfg.out_channels, H, W, device="cuda")
+        super().__init__(make_cfg(), H, W, mode, task, LR)
+        self.cid = cid
         self.hist = torch.empty(HIST, dtype=torch.float64, device="cuda")
 
     def call(self, name, iters, step0):
@@ -272,7 +203,7 @@ class Runner:
                           loss_hist=self.hist)
         torch.cuda.synchronize()
         assert adam.step_count == step0 + iters
-        self.check_noise(tag, step0 + iters - 1)
+        self.check_pin(tag, step0 + iters - 1)
         self.check_slots(tag, iters)
         if iters == 1:
             self.check_stages(tag, unflat(before[0], self.params))
@@ -283,20 +214,6 @@ class Runner:
             upd = adam_update(m, v, LR, BETAS, EPS, step0 + iters)
             delta = 2 * U * p.abs() + 8 * U * upd.abs()
             self.check_stages(tag, unflat(p + upd, self.params), unflat(delta, self.params))
-
-    def check_noise(self, tag, offset):
-        import dip_engine as de
-        zn = torch.empty_like(self.z0)
-        de.check(de.lib().dip_noise_perturb(self.z0.data_ptr(), zn.data_ptr(), SIGMA, SEED, offset, self.z0.numel(), None))
-        torch.cuda.synchronize()
-        x = SR.hwc(zn.double())
-        want = PR.zero_pad(x) if PR.pad_of(self.cfg) == "zero" else SR.reflect_pad(x)
-        pin = self.plan.buffer("L0.Pin")
-        c = self.cfg.in_channels
-        assert pin.shape[-1] == SR.stored_depth(self.cfg, 0)
-        assert torch.equal(pin[..., c:], torch.zeros_like(pin[..., c:])), "[%s] stored-depth channels not zero" % tag
-        assert torch.equal(pin[..., :c].double(), want), "[%s] L0.Pin != pad(noise stream %d): max |diff| %.3g" % (
-            tag, offset, (pin[..., :c].double() - want).abs().max().item())
 
     def check_slots(self, tag, iters):
         h = self.hist.cpu()
@@ -322,20 +239,6 @@ class Runner:
         LOSS[self.mode] = max(LOSS.get(self.mode, 0.0), abs(got - ref) / tol)
         assert abs(got - ref) <= tol, "[%s] loss slot %d = %.17g, fp64 MSE of the output %.17g, bound %.3g" % (
             tag, iters - 1, got, ref, tol)
-
-    def check_stages(self, tag, used, delta=None):
-        """every stage and gradient of the last iteration, from the engine's buffers, at parameters `used`"""
-        cfg, mode = self.cfg, self.mode
-        o = self.out.double().cpu().requires_grad_(True)
-        lo = o if self.down is None else O.downsample(o, *self.down)
-        loss = O.mse_loss(lo, self.target.double().cpu(), None if self.mask is None else self.mask.double().cpu())
-        dout = torch.autograd.grad(loss, o)[0].cuda()
-        rd = engine_src(self.plan, mode, self.out)
-        refs = SR.Refs()
-        with uncertain_params(cfg, delta) if delta is not None else contextlib.nullcontext():
-            AR.stage_forward(cfg, used, rd, mode, refs)
-            AR.stage_backward(cfg, used, rd, mode, refs, dout[0])
-        TS.check(tag, cfg, mode, self.plan, refs, self.grads, self.out)
 
 
 def print_tables():
@@ -388,7 +291,7 @@ def test_module_path_after_an_adam_step():
     buffers and gradients, checked stage by stage at the parameters it ran with (those after the first FusedAdam step)"""
     import models
     from utils.common_utils import optimize
-    cfg = TS.cfg_of("cs4")
+    cfg = E.cfg_of("cs4")
     H, W = 128, 128
     torch.manual_seed(0)
     net = models.get_net(32, "skip", "reflection", skip_n33d=128, skip_n33u=128, skip_n11=4, num_scales=5,
@@ -428,7 +331,7 @@ def test_module_path_after_an_adam_step():
     plan = list(net._dip_plans.values())[0]
     out = seen["out"].detach()
     refs = SR.Refs()
-    rd = engine_src(plan, "tf32", out)
+    rd = TS.engine_src(plan, "tf32", out)
     SR.forward(cfg, seen["params"], rd, "tf32", refs, z=z0)
     SR.backward(cfg, seen["params"], rd, "tf32", refs, seen["dout"][0])
     TS.check("module path, second closure", cfg, "tf32", plan, refs, [p.grad for p in params], out)
@@ -445,7 +348,7 @@ def test_adam_kernel_at_its_edges(hyper):
     chunks of k_adam; per-tensor gradient scales 1e-6 .. 1e2, one tensor of exact zeros (a dead bias), one with every
     other element exactly zero; steps 1, 2, 3, then 2000 and 100000; every step against the fp64 bounds above"""
     import dip_engine as de
-    cfg = TS.cfg_of("cs4")
+    cfg = E.cfg_of("cs4")
     names = [n for n, _ in O.param_layout(cfg)] + ["extra%d" % k for k in (1, 3, 2047, 2048, 2049, 4097, 147461)]
     numels = [math.prod(s) for _, s in O.param_layout(cfg)] + [1, 3, 2047, 2048, 2049, 4097, 147461]
     zero, half = names.index("L0.d1.b"), names.index("L0.d2.w")

@@ -1,43 +1,25 @@
 """The fp64 stage references of tests/stage_ref.py, composed stage by stage, against the oracle's whole network and its
-autograd gradients (CPU only).  This checks the layout, the concat rotation, the folds, the skip-conv terms and the
-upsampling adjoints of the references before they judge the engine (tests/test_stages_gpu.py)."""
-import re
-
+autograd gradients (CPU only).  This checks the layout, the concat rotation, the pads and folds, the activations and
+their derivatives, the skip-conv terms and the upsampling adjoints of the references before they judge the engine
+(tests/test_stages_gpu.py, tests/test_envelope_gpu.py).  `check_composed` is the one composition check; the zero-padded
+networks (tests/test_zero_pad_cpu.py), the other activations (tests/test_act_fun_cpu.py) and the envelope rows
+(tests/test_envelope_cpu.py) run it too."""
 import pytest
 import torch
 
 from oracle import dip_oracle as O
+import envelope_cases as E
 import stage_ref as SR
 
 H, W = 64, 96
-
-
-def cfg_of(kind):
-    if kind == "cs4":
-        return O.SkipConfig(skip_channels=4, upsample_mode="bilinear")
-    if kind == "cs128":
-        return O.SkipConfig(skip_channels=128, upsample_mode="nearest")
-    if kind == "cs0":
-        return O.SkipConfig(skip_channels=0, upsample_mode="bilinear")
-    if kind == "snail":
-        return O.SkipConfig(in_channels=3, channels=[8, 16, 32, 64, 128], skip_channels=[0, 0, 0, 4, 4])
-    if kind == "kate":
-        c = O.SkipConfig(in_channels=3, channels=[16, 32, 64, 128, 128], skip_channels=0)
-        c.downsample_mode = "avg"
-        return c
-    if kind == "modes_ingrad":   # per-scale upsampling, logits as the output, one output channel, dL/d(input)
-        return O.SkipConfig(in_channels=3, out_channels=1, skip_channels=4, need_sigmoid=False,
-                            upsample_mode=["bilinear", "nearest", "bilinear", "nearest", "nearest"])
-    raise KeyError(kind)
 
 
 def compose(cfg, params, z, target, input_grad):
     refs = SR.Refs()
 
     def src(name):
-        m = re.match(r"L(\d+)\.Pin$", name)
-        if m and int(m.group(1)) > 0:   # a level's input is the padded output of the level above
-            name = "L%d.P_d2" % (int(m.group(1)) - 1)
+        if name.startswith("L") and name.endswith(".Pin") and name != "L0.Pin":   # a level's input = the level above's P_d2
+            name = "L%d.P_d2" % (int(name[1:-4]) - 1)
         return refs[name]
 
     SR.forward(cfg, params, src, "fp64", refs, z=z)
@@ -47,15 +29,21 @@ def compose(cfg, params, z, target, input_grad):
     return refs
 
 
-@pytest.mark.parametrize("kind", ["cs4", "cs128", "cs0", "snail", "kate", "modes_ingrad"])
-def test_composed_stages_reproduce_the_oracle(kind):
-    cfg = cfg_of(kind)
-    input_grad = kind == "modes_ingrad"
+def check_composed(cfg, H, W, input_grad):
+    """cfg's stage references composed stage by stage (fp64, random affine parameters) against the oracle's output and
+    autograd gradients, dz with input_grad; with every structural check that applies to cfg"""
     params = SR.random_affine(cfg, O.init_params(cfg, seed=0, dtype=torch.float64), seed=7)
     g = torch.Generator().manual_seed(3)
     z = torch.rand(1, cfg.in_channels, H, W, generator=g, dtype=torch.float64)
     target = torch.rand(1, cfg.out_channels, H, W, generator=g, dtype=torch.float64)
     refs = compose(cfg, params, z, target, input_grad)
+    pin = refs["L0.Pin"]   # the stored depth's channels after the real ones are zeros
+    assert pin.shape[-1] == SR.stored_depth(cfg, 0) and pin[..., cfg.in_channels:].abs().sum().item() == 0
+    if cfg.pad != "reflection":   # a zero halo ring
+        assert pin[0].abs().max() == 0 and pin[-1].abs().max() == 0 and pin[:, 0].abs().max() == 0 and pin[:, -1].abs().max() == 0
+    if cfg.act_fun != "LeakyReLU":   # no jump in the derivative: no element is excluded from the backward checks
+        assert refs.excl and all(frac == 0 for frac, _ in refs.excl.values())
+        assert all(e is None or not e.any() for _, _, e in refs.d.values())
 
     p = [x.detach().clone().requires_grad_(True) for x in params]
     zz = z.clone().requires_grad_(input_grad)
@@ -74,3 +62,8 @@ def test_composed_stages_reproduce_the_oracle(kind):
             assert got.abs().max().item() == 0, name
         if name.endswith(".w") and name != "head.w":   # every conv weight gradient carries a Frobenius bound
             assert "grad:" + name in refs.conv, name
+
+
+@pytest.mark.parametrize("kind", ["cs4", "cs128", "cs0", "snail", "kate", "modes_ingrad"])
+def test_composed_stages_reproduce_the_oracle(kind):
+    check_composed(E.cfg_of(kind), H, W, kind == "modes_ingrad")

@@ -1,7 +1,8 @@
 """Zero padding (models.skip's default pad='zero', and every other value that is not 'reflection') on the host side:
 the module tree against the reference, the oracle against fixtures of the unmodified reference
-(tests/golden/make_zero_pad.py), the zero-pad stage references against the oracle's autograd, and the plan options of
-the C ABI (dip_plan_opts).  No GPU needed."""
+(tests/golden/make_zero_pad.py), the zero pad of the stage references and its adjoint, the zero-padded stage references
+composed against the oracle's autograd (tests/test_stage_ref_cpu.py's check), and the plan options of the C ABI
+(dip_plan_opts).  No GPU needed."""
 import ctypes
 import os
 
@@ -12,31 +13,16 @@ import torch
 import models
 from oracle import dip_oracle as O
 from oracle import ref_harness
-import pad_refs as PR
+import envelope_cases as E
 import stage_ref as SR
-from test_stage_ref_cpu import H, W, cfg_of
+from test_stage_ref_cpu import check_composed
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 CASES = ["skipdefault64x96_zeropad", "inpaint64x96_nearest_masked_skip128_zeropad", "restorekate64x96_avg_w16to128_zeropad"]
 
 
-def compose(cfg, params, z, target, input_grad):
-    """the stage references composed to the whole network (as tests/test_stage_ref_cpu.py), with cfg's padding"""
-    refs = SR.Refs()
-
-    def src(name):
-        if name.startswith("L") and name.endswith(".Pin") and name != "L0.Pin":   # a level's input = the level above's P_d2
-            name = "L%d.P_d2" % (int(name[1:-4]) - 1)
-        return refs[name]
-
-    PR.stage_forward(cfg, params, src, "fp64", refs, z=z)
-    out = refs["out"]
-    dout = 2.0 * (out - target[0]) / out.numel()
-    PR.stage_backward(cfg, params, src, "fp64", refs, dout, input_grad=input_grad)
-    return refs
-
-
 def oracle_cfg(g):
+    """the oracle's SkipConfig of a zero-pad or act_fun fixture"""
     chans, skips = [int(x) for x in g["chans"]], [int(x) for x in g["skips"]]
     modes = [str(m) for m in g["modes"]]
     if set(chans) == {128} and len(set(skips)) == 1:
@@ -46,11 +32,13 @@ def oracle_cfg(g):
                            skip_channels=skips)
     cfg.downsample_mode = str(g["downsample_mode"])
     cfg.pad = str(g["pad"])
+    if "act_fun" in g.files:
+        cfg.act_fun = str(g["act_fun"])
     return cfg
 
 
 def setup(g, dtype):
-    """the fixture's inputs, drawn as tests/golden/make_zero_pad.py draws them"""
+    """the fixture's inputs, drawn as tests/golden/make_zero_pad.py and make_act_fun.py draw them"""
     cfg = oracle_cfg(g)
     H_, W_ = int(g["H"]), int(g["W"])
     gen = torch.Generator().manual_seed(2)
@@ -124,9 +112,8 @@ def test_tree_equals_live_reference(pad):
     finally:
         models.allow_torch_execution(False)
     assert torch.allclose(out, rout, atol=1e-6)
-    cfg = O.SkipConfig(upsample_mode="nearest", channels=[16, 32, 64, 128, 128], skip_channels=[4] * 5)
-    cfg.pad = "zero"
-    assert torch.allclose(PR.skip_forward(O.init_params(cfg, seed=11), z, cfg).detach(), rout, atol=1e-6)
+    cfg = E.cfg_of("skipdefault", "zero")
+    assert torch.allclose(O.skip_forward(O.init_params(cfg, seed=11), z, cfg).detach(), rout, atol=1e-6)
 
 
 # ------------------------------------------------------------------------------------------------ oracle vs reference
@@ -141,7 +128,7 @@ def test_oracle_matches_reference_golden_fp64(case):
         if i == 0:
             rec["out0"], rec["grads0"] = out, [x.clone() for x in grads]
 
-    losses, _ = PR.run(cfg, params, z0, target, noises, float(g["sigma"]), float(g["lr"]), mask=mask, record=record)
+    losses, _ = O.run(cfg, params, z0, target, noises, float(g["sigma"]), float(g["lr"]), mask=mask, record=record)
     assert np.allclose(rec["out0"].numpy(), g["out0"], atol=1e-10)
     assert np.allclose(losses, g["losses"], rtol=1e-10)
     gn = np.array([x.double().norm().item() for x in rec["grads0"]])
@@ -157,56 +144,29 @@ def test_zero_pad_oracle_differs_from_reflection():
     cfg, z0, _, _, noises = setup(g, torch.float64)
     params = O.init_params(cfg, seed=0, dtype=torch.float64)
     z = z0 + noises[0] * float(g["sigma"])
-    assert np.abs(PR.skip_forward(params, z, cfg).detach().numpy() - g["out0"]).max() < 1e-10
+    assert np.abs(O.skip_forward(params, z, cfg).detach().numpy() - g["out0"]).max() < 1e-10
+    cfg.pad = "reflection"
     assert np.abs(O.skip_forward(params, z, cfg).detach().numpy() - g["out0"]).max() > 1e-4
 
 
 # ------------------------------------------------------------------------------------------------ stage references
 @pytest.mark.parametrize("kind", ["cs4", "cs128", "cs0", "snail", "kate", "modes_ingrad", "skipdefault"])
 def test_composed_zero_pad_stages_reproduce_the_oracle(kind):
-    """tests/stage_ref.py under pad_refs.padding (zero halos, folds that drop the halo), composed stage by stage, against
-    the oracle's zero-padded network and its autograd gradients (as tests/test_stage_ref_cpu.py for reflection)"""
-    if kind == "skipdefault":
-        cfg = O.SkipConfig(upsample_mode="nearest", channels=[16, 32, 64, 128, 128], skip_channels=[4] * 5)
-    else:
-        cfg = cfg_of(kind)
-    cfg.pad = "zero"
-    input_grad = kind == "modes_ingrad"
-    params = SR.random_affine(cfg, O.init_params(cfg, seed=0, dtype=torch.float64), seed=7)
-    g = torch.Generator().manual_seed(3)
-    z = torch.rand(1, cfg.in_channels, H, W, generator=g, dtype=torch.float64)
-    target = torch.rand(1, cfg.out_channels, H, W, generator=g, dtype=torch.float64)
-    refs = compose(cfg, params, z, target, input_grad)
-    pin = refs["L0.Pin"]
-    assert pin[0].abs().max() == 0 and pin[-1].abs().max() == 0 and pin[:, 0].abs().max() == 0 and pin[:, -1].abs().max() == 0
-
-    p = [x.detach().clone().requires_grad_(True) for x in params]
-    zz = z.clone().requires_grad_(input_grad)
-    out = PR.skip_forward(p, zz, cfg)
-    assert (refs["out"] - out.detach()[0]).abs().max().item() < 1e-12
-    grads = torch.autograd.grad(O.mse_loss(out, target), p + ([zz] if input_grad else []))
-    names = [n for n, _ in O.param_layout(cfg)] + (["dz"] if input_grad else [])
-    gmax = max(gr.abs().max().item() for gr in grads)
-    for name, gr in zip(names, grads):
-        got = refs[name if name == "dz" else "grad:" + name].reshape(gr.shape)
-        err = (got - gr).abs().max().item()
-        assert err <= max(1e-10 * gr.abs().max().item(), 1e-13 * gmax), (name, err, gr.abs().max().item())
+    """tests/stage_ref.py with zero padding (zero halos, folds that drop the halo), composed stage by stage, against the
+    oracle's zero-padded network and its autograd gradients (tests/test_stage_ref_cpu.py's check)"""
+    check_composed(E.cfg_of(kind, "zero"), 64, 96, kind == "modes_ingrad")
 
 
-def test_padding_swaps_only_for_zero_pad():
-    """reflection configurations keep the references' own functions; zero padding swaps them only inside the context"""
-    cfg = O.SkipConfig()
-    saved = (O._conv, SR.reflect_pad, SR.fold)
-    with PR.padding(cfg):
-        assert (O._conv, SR.reflect_pad, SR.fold) == saved
-    cfg.pad = "zero"
+def test_zero_pad_and_its_fold():
+    """stage_ref pads every value of pad other than 'reflection' with a zero halo, and its fold keeps the interior"""
     x = torch.rand(4, 6, 3, dtype=torch.float64)
-    with PR.padding(cfg):
-        p = SR.reflect_pad(x)
+    assert SR.padding(O.SkipConfig()) == (SR.reflect_pad, SR.fold)
+    for pad in ("zero", "replication"):
+        p, fold = SR.padding(E.cfg_of("cs4", pad))
+        y = p(x)
         ring = torch.ones(6, 8, 1, dtype=torch.bool)
         ring[1:-1, 1:-1] = False
-        assert torch.equal(p[1:-1, 1:-1], x) and (p * ring).abs().max() == 0 and torch.equal(SR.fold(p), x)
-    assert (O._conv, SR.reflect_pad, SR.fold) == saved
+        assert torch.equal(y[1:-1, 1:-1], x) and (y * ring).abs().max() == 0 and torch.equal(fold(y), x)
 
 
 # ------------------------------------------------------------------------------------------------ C ABI
