@@ -171,6 +171,69 @@ enum HbmId { H_INPUT_PAD = 0, H_NOISE, H_SKINNY_FWD, H_BN_ACT_WRITE, H_BN_ACT_HE
     stmt;                                                                                  \
   } while (0)
 
+// ------------------------------------------------------------------------------------------------ weight pack and split-K sum
+// Every convolution, in the plan and in the single-op entry points, packs its weights through k_pack_table and sums its
+// split-K weight-gradient partials through k_wgrad_unpack_table.
+struct PackEntry {
+  const float* w; float* dst_f; float* dst_d;
+  int N, C, k, rot, n_rows, c_pad, c_rows;
+  int Ctot, coff;   // weight has Ctot input channels; this entry packs engine channels [coff, coff + C)
+  int s2;           // dgrad pack of a stride-2 3x3 conv: taps in sub-pixel phase order (kS2Taps), not flipped
+  int bf16;         // packs hold bf16 (same buffers); the fprop pack then has rows of c_pad16 (multiple of 64) channels
+  int c_pad16;
+  int n_pad;        // columns of the dgrad pack: N rounded up to 32 (bf16: to 64)
+};
+// packed tap t of the 4-phase stride-2 dgrad -> filter tap r * 3 + s.  Phase (a, b) = parity of the padded gradient pixel;
+// its taps are r in {2, 0} (a = 0: dY rows i-1, i) or {1} (a = 1), same for s.  Phases in the order (0,0) (0,1) (1,0) (1,1).
+__constant__ int kS2Taps[9] = {2 * 3 + 2, 2 * 3 + 0, 0 * 3 + 2, 0 * 3 + 0,   // (0,0): (r', s') = (0,0) (0,1) (1,0) (1,1)
+                               2 * 3 + 1, 0 * 3 + 1,                           // (0,1): s = 1
+                               1 * 3 + 2, 1 * 3 + 0,                           // (1,0): r = 1
+                               1 * 3 + 1};                                     // (1,1)
+__global__ void k_pack_table(const PackEntry* __restrict__ tab) {
+  pdl_enter();
+  const PackEntry e = tab[blockIdx.y];
+  const int taps = e.k * e.k;
+  const int c_pad = e.bf16 ? e.c_pad16 : e.c_pad;
+  __nv_bfloat16* const f16 = reinterpret_cast<__nv_bfloat16*>(e.dst_f);
+  __nv_bfloat16* const d16 = reinterpret_cast<__nv_bfloat16*>(e.dst_d);
+  const long long nf = e.dst_f != nullptr ? (long long)taps * e.n_rows * c_pad : 0;
+  const long long nd = e.dst_d != nullptr ? (long long)taps * e.c_rows * e.n_pad : 0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nf + nd; i += (long long)gridDim.x * blockDim.x) {
+    if (i < nf) {
+      const int c = (int)(i % c_pad), n = (int)((i / c_pad) % e.n_rows), tap = (int)(i / ((long long)c_pad * e.n_rows));
+      float v = 0.f;
+      if (n < e.N && c < e.C) v = e.w[((long long)n * e.Ctot + (c + e.coff + e.rot) % e.Ctot) * taps + tap];
+      if (e.bf16) f16[i] = __float2bfloat16_rn(v); else e.dst_f[i] = v;
+    } else {
+      const long long j = i - nf;
+      const int n = (int)(j % e.n_pad), c = (int)((j / e.n_pad) % e.c_rows), tapf = (int)(j / ((long long)e.n_pad * e.c_rows));
+      const int tap = e.s2 ? kS2Taps[tapf] : taps - 1 - tapf;
+      float v = 0.f;
+      if (n < e.N && c < e.C) v = e.w[((long long)n * e.Ctot + (c + e.coff + e.rot) % e.Ctot) * taps + tap];
+      if (e.bf16) d16[j] = __float2bfloat16_rn(v); else e.dst_d[j] = v;
+    }
+  }
+}
+// split-K partials [ks][tap][128][cols] of a weight gradient -> OIHW gradient, one entry per conv (the tensor-core plan
+// sums all of them in one launch per backward pass, the fp32-mode plan and the single-op wgrad one entry after each
+// wgrad); the split-K slices are summed in index order, so the gradient is the same on every run
+struct UnpackEntry {
+  const float* acc; float* dw;
+  int N, C, taps, rot, cols, Ctot, coff, ks;   // cols: row stride of the partials (ConvOp::part_cols)
+};
+__global__ void k_wgrad_unpack_table(const UnpackEntry* __restrict__ tab) {
+  pdl_enter();
+  const UnpackEntry e = tab[blockIdx.y];
+  const int total = e.N * e.C * e.taps;   // dw elements this entry owns: (n, engine channel c, tap)
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+    const int tap = i % e.taps, c = (i / e.taps) % e.C, n = i / (e.taps * e.C);
+    const size_t split = (size_t)e.taps * 128 * e.cols;
+    const float* src = e.acc + ((size_t)tap * 128 + n) * e.cols + c;
+    float v = 0.f;
+    for (int k = 0; k < e.ks; ++k) v += src[k * split];
+    e.dw[((size_t)n * e.Ctot + (c + e.coff + e.rot) % e.Ctot) * e.taps + tap] = v;
+  }
+}
 // ------------------------------------------------------------------------------------------------ conv op
 // CTAs per pixel tile (output channels split across them) for launches with fewer tiles than SMs: n_rows % (32 * split) == 0
 static int pick_nsplit(int tiles, int n_rows) {
@@ -204,26 +267,27 @@ struct ConvOp {
   bool bf16 = false;
   int c_pad16 = 0;                                   // fprop K extent per tap in bf16 (multiple of 64)
   const uint16_t* in16 = nullptr; int in_ld16 = 0;   // twin of `in`
-  const uint16_t* dg_in16 = nullptr;                 // twin of dg_in (ld 128)
-  const uint16_t* wg_dy16 = nullptr;                 // twin of wg_dy (ld 128)
-  // forward
+  const uint16_t* dy16 = nullptr;                    // twin of `dy`
+  // forward: in -> out [out_h][out_w][N]
   const float* in = nullptr; int in_rows = 0, in_cols = 0, in_ld = 0; int offx = 0, offy = 0;
   float* out = nullptr; int out_h = 0, out_w = 0;
   double* stats = nullptr;
   float* wp_f = nullptr; float* wp_d = nullptr;
-  float* wacc = nullptr;   // plan-owned weight-gradient partials [ksplits][tap][128][wg_cols()] (tensor-core path)
-  // dgrad: dg_in [dg_in_h][dg_in_w][128] -> dg_out [dg_out_h][dg_out_w][C]
+  // dY [out_h][out_w][N]: the gradient of `out`, read by the dgrad and the wgrad
+  const float* dy = nullptr;
+  // dgrad: dY -> dg_out [dg_out_h][dg_out_w][C]
   bool has_dgrad = false;
-  bool dg_s2 = false;   // tensor-core dgrad of a stride-2 3x3 conv as its 4 sub-pixel phases (dg_in = dY [h][w][128], not zero-stuffed)
-  const float* dg_in = nullptr; int dg_in_h = 0, dg_in_w = 0;
+  bool dg_s2 = false;   // tensor-core dgrad of a stride-2 3x3 conv as its 4 sub-pixel phases (reads dY, not zero-stuffed)
+  const float* zs = nullptr;   // fp32 mode, stride 2: the dgrad reads dY zero-stuffed to [2 out_h][2 out_w][N] instead
   float* dg_out = nullptr; int dg_out_h = 0, dg_out_w = 0; int dg_off = 0;
-  // wgrad: dY [wg_h][wg_w][128]
-  const float* wg_dy = nullptr; int wg_h = 0, wg_w = 0;
+  // wgrad: split-K partials [part_ks][tap][128][part_cols] (the tensor-core plan gives every conv its own; the fp32-mode
+  // plan shares one area between all convs), summed into the gradient by one UnpackEntry per conv
+  float* partial = nullptr;
+  const UnpackEntry* unpack = nullptr;   // launched right after the wgrad; nullptr: the plan sums every entry at the end
   // param slots
   int p_w = -1, p_b = -1;
   TcConvParams fp{}, dg{};   // what the launches run: the general form, or its stride-1 3x3 patch form
   TcWgradParams wg{};
-  int simt_ksplits = 1;
 
   void set_shapes() {
     c_pad = round_up(C, 32);
@@ -235,7 +299,6 @@ struct ConvOp {
   }
   size_t wp_f_elems() const { return (size_t)k * k * Np * c_pad; }
   size_t wp_d_elems() const { return (size_t)k * k * crows * n_pad; }
-  size_t wacc_elems() const { return (size_t)tc_ksplits() * k * k * 128 * wg_cols(); }
   // accumulator columns of the tensor-core weight gradient (wgmma N, row stride of its partials): c_pad, except 136 for
   // 128 < C <= 136 (the 128 + 4 channel concat convs), which would otherwise multiply 24 zero columns of every 160
   int wg_cols() const { return C > 128 && C <= 136 ? 136 : c_pad; }
@@ -243,13 +306,25 @@ struct ConvOp {
   // slice, so more items than SMs only add traffic).  A constant, not the device's count: the plan's size is known
   // without a device, and the split -- hence the summation order of the gradient -- is the same on every device.
   int tc_ksplits() const {
-    const int blocks = wg_h * ((wg_w + kWgradKp - 1) / kWgradKp);
+    const int blocks = out_h * ((out_w + kWgradKp - 1) / kWgradKp);
     int ks = static_cast<int>(kNumSms) / (k * k);
     if (ks > blocks) ks = blocks;
     return ks < 1 ? 1 : ks;
   }
-  size_t partial_elems(int prec) const {
-    return is_tc(prec) ? wacc_elems() : (size_t)simt_ksplits * k * k * 128 * c_pad;
+  int simt_ksplits() const { return out_h < 64 ? out_h : 64; }   // row ranges of the SIMT weight gradient
+  int part_ks(int prec) const { return is_tc(prec) ? tc_ksplits() : simt_ksplits(); }
+  int part_cols(int prec) const { return is_tc(prec) ? wg_cols() : c_pad; }
+  size_t partial_elems(int prec) const { return (size_t)part_ks(prec) * k * k * 128 * part_cols(prec); }
+  PackEntry pack_entry(const float* w) const {
+    PackEntry e{};
+    e.w = w; e.dst_f = do_fprop ? wp_f : nullptr; e.dst_d = has_dgrad ? wp_d : nullptr;
+    e.N = N; e.C = C; e.k = k; e.rot = rot; e.n_rows = Np; e.c_pad = c_pad; e.c_rows = crows;
+    e.Ctot = Ctot; e.coff = coff; e.s2 = dg_s2 ? 1 : 0;
+    e.bf16 = bf16 ? 1 : 0; e.c_pad16 = c_pad16; e.n_pad = bf16 ? n_pad16 : n_pad;
+    return e;
+  }
+  UnpackEntry unpack_entry(int prec, float* dw) const {
+    return UnpackEntry{partial, dw, N, C, k * k, rot, part_cols(prec), Ctot, coff, part_ks(prec)};
   }
 
   // Replaces the general form g of a stride-1 3x3 conv by its patch form (tc_conv_patch_kernel): the same tiles, weights,
@@ -267,90 +342,76 @@ struct ConvOp {
     g = t;
     return 0;
   }
-  int build_tc(float* partial) {
+  int build_tc() {
     // ---- fprop
     int bw, bh;
-    pick_tile(out_w, out_h, &bw, &bh);
     fp = TcConvParams{};
     if (do_fprop) {
-    DIP_CHECK(bf16 ? map_act5(&fp.tmA, in16, in_rows, in_cols, in_ld16, C, stride, bw, bh, true)
-                   : map_act5(&fp.tmA, in, in_rows, in_cols, in_ld, C, stride, bw, bh));
-    fp.n_split = pick_nsplit(((out_w + bw - 1) / bw) * ((out_h + bh - 1) / bh), Np);
-    DIP_CHECK(map_w2(&fp.tmB, wp_f, k * k * Np, bf16 ? c_pad16 : c_pad, Np / fp.n_split, bf16));
-    DIP_CHECK(map_act3(&fp.tmD, out, out_h, out_w, N, N, bw, bh));
-    fp.tiles_x = (out_w + bw - 1) / bw; fp.tiles_y = (out_h + bh - 1) / bh;
-    fp.bw = bw; fp.bh = bh; fp.out_w = out_w; fp.out_h = out_h;
-    fp.kh = fp.kw = k; fp.stride = stride; fp.offx = offx; fp.offy = offy;
-    fp.bf16 = bf16 ? 1 : 0;
-    fp.kblocks = bf16 ? c_pad16 / 64 : c_pad / 32;
-    fp.n_mma = Np / fp.n_split; fp.n_chunks = (fp.n_mma + 31) / 32;
-    fp.n_valid = N;
-    fp.bias = nullptr; fp.stats = stats; fp.stats_ld = N;
-    fit_stages(fp);
+      pick_tile(out_w, out_h, &bw, &bh);
+      DIP_CHECK(bf16 ? map_act5(&fp.tmA, in16, in_rows, in_cols, in_ld16, C, stride, bw, bh, true)
+                     : map_act5(&fp.tmA, in, in_rows, in_cols, in_ld, C, stride, bw, bh));
+      fp.n_split = pick_nsplit(((out_w + bw - 1) / bw) * ((out_h + bh - 1) / bh), Np);
+      DIP_CHECK(map_w2(&fp.tmB, wp_f, k * k * Np, bf16 ? c_pad16 : c_pad, Np / fp.n_split, bf16));
+      DIP_CHECK(map_act3(&fp.tmD, out, out_h, out_w, N, N, bw, bh));
+      fp.tiles_x = (out_w + bw - 1) / bw; fp.tiles_y = (out_h + bh - 1) / bh;
+      fp.bw = bw; fp.bh = bh; fp.out_w = out_w; fp.out_h = out_h;
+      fp.kh = fp.kw = k; fp.stride = stride; fp.offx = offx; fp.offy = offy;
+      fp.bf16 = bf16 ? 1 : 0;
+      fp.kblocks = bf16 ? c_pad16 / 64 : c_pad / 32;
+      fp.n_mma = Np / fp.n_split; fp.n_chunks = (fp.n_mma + 31) / 32;
+      fp.n_valid = N;
+      fp.bias = nullptr; fp.stats = stats; fp.stats_ld = N;
+      fit_stages(fp);
+      if (k == 3 && stride == 1)
+        DIP_CHECK(bf16 ? patch_form(fp, in16, in_rows, in_cols, in_ld16, C) : patch_form(fp, in, in_rows, in_cols, in_ld, C));
     }
-    if (do_fprop && k == 3 && stride == 1)
-      DIP_CHECK(bf16 ? patch_form(fp, in16, in_rows, in_cols, in_ld16, C) : patch_form(fp, in, in_rows, in_cols, in_ld, C));
-    // ---- dgrad
-    if (has_dgrad && dg_s2) {
-      // phase grid: (dg_out_h / 2) x (dg_out_w / 2) positions per parity class of the padded gradient
-      const int gh = dg_out_h / 2, gw = dg_out_w / 2;
+    // ---- dgrad: K = the N channels of dY.  Stride 2: the 4 sub-pixel phases over the (dg_out_h / 2) x (dg_out_w / 2)
+    // positions of each parity class of the padded gradient
+    dg = TcConvParams{};
+    if (has_dgrad) {
+      const int gh = dg_s2 ? dg_out_h / 2 : dg_out_h, gw = dg_s2 ? dg_out_w / 2 : dg_out_w;
       pick_tile(gw, gh, &bw, &bh);
-      dg = TcConvParams{};
-      DIP_CHECK(bf16 ? map_act5(&dg.tmA, dg_in16, dg_in_h, dg_in_w, N, N, 1, bw, bh, true)
-                     : map_act5(&dg.tmA, dg_in, dg_in_h, dg_in_w, N, N, 1, bw, bh));
-      dg.n_split = pick_nsplit(4 * ((gw + bw - 1) / bw) * ((gh + bh - 1) / bh), crows);
-      DIP_CHECK(map_w2(&dg.tmB, wp_d, k * k * crows, bf16 ? n_pad16 : n_pad, crows / dg.n_split, bf16));
-      DIP_CHECK(map_act5(&dg.tmD, dg_out, dg_out_h, dg_out_w, dg_ld, C, 2, bw, bh));   // parity view of the padded gradient
+      DIP_CHECK(bf16 ? map_act5(&dg.tmA, dy16, out_h, out_w, N, N, 1, bw, bh, true)
+                     : map_act5(&dg.tmA, dy, out_h, out_w, N, N, 1, bw, bh));
       dg.tiles_x = (gw + bw - 1) / bw; dg.tiles_y = (gh + bh - 1) / bh;
-      dg.bw = bw; dg.bh = bh; dg.out_w = gw; dg.out_h = gh;
-      dg.kh = dg.kw = 2; dg.stride = 1; dg.offx = dg.offy = -1;
-      dg.nphase = 4;
-      int t0 = 0;
-      for (int a = 0; a < 2; ++a)
-        for (int b = 0; b < 2; ++b) {
-          TcConvParams::Phase& q = dg.phs[a * 2 + b];
-          q.kh = 2 - a; q.kw = 2 - b; q.offy = a == 0 ? -1 : 0; q.offx = b == 0 ? -1 : 0; q.tap0 = t0; q.opx = b; q.opy = a;
-          t0 += q.kh * q.kw;
-        }
-      dg.bf16 = bf16 ? 1 : 0;
-      dg.kblocks = bf16 ? n_pad16 / 64 : n_pad / 32;   // K = the N channels of dY
-      dg.n_mma = crows / dg.n_split; dg.n_chunks = (dg.n_mma + 31) / 32;
-      dg.bias = nullptr; dg.stats = nullptr; dg.stats_ld = 0;
-      fit_stages(dg);
-    } else if (has_dgrad) {
-      pick_tile(dg_out_w, dg_out_h, &bw, &bh);
-      dg = TcConvParams{};
-      DIP_CHECK(bf16 ? map_act5(&dg.tmA, dg_in16, dg_in_h, dg_in_w, N, N, 1, bw, bh, true)
-                     : map_act5(&dg.tmA, dg_in, dg_in_h, dg_in_w, N, N, 1, bw, bh));
-      dg.n_split = pick_nsplit(((dg_out_w + bw - 1) / bw) * ((dg_out_h + bh - 1) / bh), crows);
+      dg.n_split = pick_nsplit((dg_s2 ? 4 : 1) * dg.tiles_x * dg.tiles_y, crows);
       DIP_CHECK(map_w2(&dg.tmB, wp_d, k * k * crows, bf16 ? n_pad16 : n_pad, crows / dg.n_split, bf16));
-      DIP_CHECK(map_act3(&dg.tmD, dg_out, dg_out_h, dg_out_w, dg_ld, C, bw, bh));
-      dg.tiles_x = (dg_out_w + bw - 1) / bw; dg.tiles_y = (dg_out_h + bh - 1) / bh;
-      dg.bw = bw; dg.bh = bh; dg.out_w = dg_out_w; dg.out_h = dg_out_h;
-      dg.kh = dg.kw = k; dg.stride = 1; dg.offx = dg.offy = dg_off;
+      DIP_CHECK(dg_s2 ? map_act5(&dg.tmD, dg_out, dg_out_h, dg_out_w, dg_ld, C, 2, bw, bh)   // parity view of the padded gradient
+                      : map_act3(&dg.tmD, dg_out, dg_out_h, dg_out_w, dg_ld, C, bw, bh));
+      dg.bw = bw; dg.bh = bh; dg.out_w = gw; dg.out_h = gh;
+      dg.stride = 1;
+      if (dg_s2) {
+        dg.kh = dg.kw = 2; dg.offx = dg.offy = -1;
+        dg.nphase = 4;
+        int t0 = 0;
+        for (int a = 0; a < 2; ++a)
+          for (int b = 0; b < 2; ++b) {
+            TcConvParams::Phase& q = dg.phs[a * 2 + b];
+            q.kh = 2 - a; q.kw = 2 - b; q.offy = a == 0 ? -1 : 0; q.offx = b == 0 ? -1 : 0; q.tap0 = t0; q.opx = b; q.opy = a;
+            t0 += q.kh * q.kw;
+          }
+      } else {
+        dg.kh = dg.kw = k; dg.offx = dg.offy = dg_off;
+      }
       dg.bf16 = bf16 ? 1 : 0;
-      dg.kblocks = bf16 ? n_pad16 / 64 : n_pad / 32;   // K = the N channels of dY
+      dg.kblocks = bf16 ? n_pad16 / 64 : n_pad / 32;
       dg.n_mma = crows / dg.n_split; dg.n_chunks = (dg.n_mma + 31) / 32;
-      dg.bias = nullptr; dg.stats = nullptr; dg.stats_ld = 0;
       fit_stages(dg);
+      if (!dg_s2 && k == 3)
+        DIP_CHECK(bf16 ? patch_form(dg, dy16, out_h, out_w, N, N) : patch_form(dg, dy, out_h, out_w, N, N));
     }
-    if (has_dgrad && !dg_s2 && k == 3)
-      DIP_CHECK(bf16 ? patch_form(dg, dg_in16, dg_in_h, dg_in_w, N, N) : patch_form(dg, dg_in, dg_in_h, dg_in_w, N, N));
     // ---- wgrad
     wg = TcWgradParams{};
     if (!do_wgrad) return 0;
     wg.bf16 = bf16 ? 1 : 0;
-    if (bf16) {
-      DIP_CHECK(map_act3(&wg.tmY, wg_dy16, wg_h, wg_w, N, N, kWgradKp, 1, true));
-      DIP_CHECK(map_act5(&wg.tmX, in16, in_rows, in_cols, in_ld16, C, stride, kWgradKp, 1, true));
-    } else {
-      DIP_CHECK(map_act3(&wg.tmY, wg_dy, wg_h, wg_w, N, N, kWgradKp, 1));
-      DIP_CHECK(map_act5(&wg.tmX, in, in_rows, in_cols, in_ld, C, stride, kWgradKp, 1));
-    }
+    DIP_CHECK(bf16 ? map_act3(&wg.tmY, dy16, out_h, out_w, N, N, kWgradKp, 1, true)
+                   : map_act3(&wg.tmY, dy, out_h, out_w, N, N, kWgradKp, 1));
+    DIP_CHECK(bf16 ? map_act5(&wg.tmX, in16, in_rows, in_cols, in_ld16, C, stride, kWgradKp, 1, true)
+                   : map_act5(&wg.tmX, in, in_rows, in_cols, in_ld, C, stride, kWgradKp, 1));
     wg.partial = partial;
     wg.kh = wg.kw = k; wg.stride = stride; wg.offx = offx; wg.offy = offy;
-    wg.px_blocks_x = (wg_w + kWgradKp - 1) / kWgradKp;
-    wg.px_blocks = wg_h * wg.px_blocks_x;
+    wg.px_blocks_x = (out_w + kWgradKp - 1) / kWgradKp;
+    wg.px_blocks = out_h * wg.px_blocks_x;
     wg.c_chunks = bf16 ? c_pad16 / 64 : c_pad / 32;
     wg.n_cols = wg_cols();
     wg.ksplits = tc_ksplits();
@@ -384,7 +445,8 @@ struct ConvOp {
       DIP_CUDA(tc_conv_launch(dg, g_num_sms, s));
     } else {
       SimtConvArgs a{};
-      a.A = dg_in; a.a_h = dg_in_h; a.a_w = dg_in_w; a.a_ld = N; a.a_c = N;
+      a.A = zs != nullptr ? zs : dy; a.a_h = zs != nullptr ? 2 * out_h : out_h; a.a_w = zs != nullptr ? 2 * out_w : out_w;
+      a.a_ld = N; a.a_c = N;
       a.Wp = wp_d; a.n_rows = crows; a.c_pad = n_pad;
       a.D = dg_out; a.d_h = dg_out_h; a.d_w = dg_out_w; a.d_ld = dg_ld; a.d_c = C;
       a.kh = a.kw = k; a.stride = 1; a.offx = a.offy = dg_off; a.bias = nullptr;
@@ -393,99 +455,31 @@ struct ConvOp {
     }
     return 0;
   }
-  int run_wgrad(int prec, float* partial, float* dw, cudaStream_t s) {
+  // Every split-K work item of the weight gradient writes its own slice of `partial`; `unpack` (when set) then sums the
+  // slices into the OIHW gradient.
+  int run_wgrad(int prec, cudaStream_t s) {
     static const bool dbg_skip = getenv("DIP_DBG_SKIP_WGRAD") != nullptr;   // timing diagnostic only: gradients are wrong
     if (dbg_skip) return 0;
-    int ks;
     if (is_tc(prec)) {
-      // every split-K work item writes its own partial slice.  Plan-owned partials (wacc) are summed and unpacked to
-      // OIHW by one table kernel at the end of the backward pass; single-op entry points reduce here.
-      TcWgradParams p = wg;
-      p.partial = wacc != nullptr ? wacc : partial;
-      {
-        TimeScope ts(timer, 2, alg_flops(), s);
-        DIP_CUDA(tc_wgrad_launch(p, s));
-      }
-      if (wacc != nullptr) return 0;
-      launch_wgrad_reduce(partial, p.ksplits, N, C, k, k, rot, p.n_cols, dw, s, Ctot, coff);
-      DIP_CUDA(cudaGetLastError());
-      return 0;
+      TimeScope ts(timer, 2, alg_flops(), s);
+      DIP_CUDA(tc_wgrad_launch(wg, s));
     } else {
       SimtWgradArgs a{};
-      a.dY = wg_dy; a.h = wg_h; a.w = wg_w; a.dy_ld = N; a.n = N;
+      a.dY = dy; a.h = out_h; a.w = out_w; a.dy_ld = N; a.n = N;
       a.X = in; a.x_h = in_rows; a.x_w = in_cols; a.x_ld = in_ld; a.x_c = C;
       a.kh = a.kw = k; a.stride = stride; a.offx = offx; a.offy = offy;
-      a.partial = partial; a.c_pad = c_pad; a.ksplits = ks = simt_ksplits;
+      a.partial = partial; a.c_pad = c_pad; a.ksplits = simt_ksplits();
       launch_simt_wgrad(a, s);
     }
-    HBM_T(timer, H_WGRAD_REDUCE, 0, ((double)ks + 1.0) * k * k * 128.0 * c_pad * sizeof(float), s,
-          launch_wgrad_reduce(partial, ks, N, C, k, k, rot, c_pad, dw, s, Ctot, coff));
+    if (unpack != nullptr)
+      HBM_T(timer, H_WGRAD_REDUCE, 0, ((double)part_ks(prec) + 1.0) * k * k * 128.0 * part_cols(prec) * sizeof(float), s,
+            launch_k(k_wgrad_unpack_table, dim3(64, 1), dim3(256), 0, s, 1, unpack));
     DIP_CUDA(cudaGetLastError());
     return 0;
   }
 };
 
 // ------------------------------------------------------------------------------------------------ table kernels
-struct PackEntry {
-  const float* w; float* dst_f; float* dst_d;
-  int N, C, k, rot, n_rows, c_pad, c_rows;
-  int Ctot, coff;   // weight has Ctot input channels; this entry packs engine channels [coff, coff + C)
-  int s2;           // dgrad pack of a stride-2 3x3 conv: taps in sub-pixel phase order (kS2Taps), not flipped
-  int bf16;         // packs hold bf16 (same buffers); the fprop pack then has rows of c_pad16 (multiple of 64) channels
-  int c_pad16;
-  int n_pad;        // columns of the dgrad pack: N rounded up to 32 (bf16: to 64)
-};
-// packed tap t of the 4-phase stride-2 dgrad -> filter tap r * 3 + s.  Phase (a, b) = parity of the padded gradient pixel;
-// its taps are r in {2, 0} (a = 0: dY rows i-1, i) or {1} (a = 1), same for s.  Phases in the order (0,0) (0,1) (1,0) (1,1).
-__constant__ int kS2Taps[9] = {2 * 3 + 2, 2 * 3 + 0, 0 * 3 + 2, 0 * 3 + 0,   // (0,0): (r', s') = (0,0) (0,1) (1,0) (1,1)
-                               2 * 3 + 1, 0 * 3 + 1,                           // (0,1): s = 1
-                               1 * 3 + 2, 1 * 3 + 0,                           // (1,0): r = 1
-                               1 * 3 + 1};                                     // (1,1)
-__global__ void k_pack_table(const PackEntry* __restrict__ tab) {
-  pdl_enter();
-  const PackEntry e = tab[blockIdx.y];
-  const int taps = e.k * e.k;
-  const int c_pad = e.bf16 ? e.c_pad16 : e.c_pad;
-  __nv_bfloat16* const f16 = reinterpret_cast<__nv_bfloat16*>(e.dst_f);
-  __nv_bfloat16* const d16 = reinterpret_cast<__nv_bfloat16*>(e.dst_d);
-  const long long nf = e.dst_f != nullptr ? (long long)taps * e.n_rows * c_pad : 0;
-  const int n_pad = e.n_pad > 0 ? e.n_pad : 128;
-  const long long nd = e.dst_d != nullptr ? (long long)taps * e.c_rows * n_pad : 0;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nf + nd; i += (long long)gridDim.x * blockDim.x) {
-    if (i < nf) {
-      const int c = (int)(i % c_pad), n = (int)((i / c_pad) % e.n_rows), tap = (int)(i / ((long long)c_pad * e.n_rows));
-      float v = 0.f;
-      if (n < e.N && c < e.C) v = e.w[((long long)n * e.Ctot + (c + e.coff + e.rot) % e.Ctot) * taps + tap];
-      if (e.bf16) f16[i] = __float2bfloat16_rn(v); else e.dst_f[i] = v;
-    } else {
-      const long long j = i - nf;
-      const int n = (int)(j % n_pad), c = (int)((j / n_pad) % e.c_rows), tapf = (int)(j / ((long long)n_pad * e.c_rows));
-      const int tap = e.s2 ? kS2Taps[tapf] : taps - 1 - tapf;
-      float v = 0.f;
-      if (n < e.N && c < e.C) v = e.w[((long long)n * e.Ctot + (c + e.coff + e.rot) % e.Ctot) * taps + tap];
-      if (e.bf16) d16[j] = __float2bfloat16_rn(v); else e.dst_d[j] = v;
-    }
-  }
-}
-// partials [ks][tap][128][cols] of all tensor-core weight gradients -> OIHW gradients (one launch per backward pass);
-// the split-K slices are summed in index order, so the gradient is the same on every run
-struct UnpackEntry {
-  const float* acc; float* dw;
-  int N, C, taps, rot, cols, Ctot, coff, ks;   // cols: row stride of the partials (ConvOp::wg_cols)
-};
-__global__ void k_wgrad_unpack_table(const UnpackEntry* __restrict__ tab) {
-  pdl_enter();
-  const UnpackEntry e = tab[blockIdx.y];
-  const int total = e.N * e.C * e.taps;   // dw elements this entry owns: (n, engine channel c, tap)
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-    const int tap = i % e.taps, c = (i / e.taps) % e.C, n = i / (e.taps * e.C);
-    const size_t split = (size_t)e.taps * 128 * e.cols;
-    const float* src = e.acc + ((size_t)tap * 128 + n) * e.cols + c;
-    float v = 0.f;
-    for (int k = 0; k < e.ks; ++k) v += src[k * split];
-    e.dw[((size_t)n * e.Ctot + (c + e.coff + e.rot) % e.Ctot) * e.taps + tap] = v;
-  }
-}
 struct CvtEntry {
   const double* src; float* dst; int n, rot;
   int row, row_ld;   // dst rows of `row` elements come from accumulator rows of `row_ld` (0: contiguous)
@@ -912,16 +906,12 @@ static int build_plan(dip_plan* P, Arena& A) {
     a.has_dgrad = l > 0 || d.input_grad != 0;
     a.dg_ld = v.Cin;   // level 0: stored depth (>= the conv's real input depth)
     a.dg_s2 = is_tc(prec);   // (fp32 mode and 'avg' take the zero-stuffed stride-1 dgrad)
-    if (a.dg_s2) { a.dg_in = v.dRaw_d1; a.dg_in_h = v.h; a.dg_in_w = v.w; }
-    else { a.dg_in = v.ZS; a.dg_in_h = v.H; a.dg_in_w = v.W; }
+    a.dy = v.dRaw_d1; a.dy16 = v.dRaw_d1_16; a.zs = a.dg_s2 ? nullptr : v.ZS;
     a.dg_out = v.dPin; a.dg_out_h = v.H + 2; a.dg_out_w = v.W + 2; a.dg_off = -2;
-    a.wg_dy = v.dRaw_d1; a.wg_h = v.h; a.wg_w = v.w;
-    a.in16 = v.Pin16; a.in_ld16 = v.Pin_ld16; a.dg_in16 = v.dRaw_d1_16; a.wg_dy16 = v.dRaw_d1_16;
+    a.in16 = v.Pin16; a.in_ld16 = v.Pin_ld16;
     if (avg) {   // stride-1 conv at the level's full resolution; pooling is a separate pass (fwd_level / bwd_level)
       a.stride = 1; a.out = v.rawF; a.out_h = v.H; a.out_w = v.W; a.stats = nullptr;
-      a.dg_s2 = false; a.dg_in = v.dRawF; a.dg_in_h = v.H; a.dg_in_w = v.W;
-      a.wg_dy = v.dRawF; a.wg_h = v.H; a.wg_w = v.W;
-      a.dg_in16 = v.dRawF16; a.wg_dy16 = v.dRawF16;
+      a.dg_s2 = false; a.dy = v.dRawF; a.dy16 = v.dRawF16; a.zs = nullptr;
     }
     // down2: P_d1 -> raw_d2
     ConvOp& b = v.d2;
@@ -929,27 +919,27 @@ static int build_plan(dip_plan* P, Arena& A) {
     b.in = v.P_d1; b.in_rows = v.h + 2; b.in_cols = v.w + 2; b.in_ld = v.nd; b.offx = b.offy = 0;
     b.out = v.raw_d2; b.out_h = v.h; b.out_w = v.w; b.stats = v.bn_d2.fwd;
     b.has_dgrad = true;
-    b.dg_in = v.dRaw_d2; b.dg_in_h = v.h; b.dg_in_w = v.w; b.dg_out = v.dP_d1; b.dg_out_h = v.h + 2; b.dg_out_w = v.w + 2; b.dg_off = -2;
-    b.wg_dy = v.dRaw_d2; b.wg_h = v.h; b.wg_w = v.w;
-    b.in16 = v.P_d1_16; b.in_ld16 = v.nd; b.dg_in16 = v.dRaw_d2_16; b.wg_dy16 = v.dRaw_d2_16;
+    b.dy = v.dRaw_d2; b.dy16 = v.dRaw_d2_16;
+    b.dg_out = v.dP_d1; b.dg_out_h = v.h + 2; b.dg_out_w = v.w + 2; b.dg_off = -2;
+    b.in16 = v.P_d1_16; b.in_ld16 = v.nd;
     // up: P_cat -> raw_u
     ConvOp& c = v.up;
     c.set_shapes();
     c.in = v.P_cat; c.in_rows = v.H + 2; c.in_cols = v.W + 2; c.in_ld = v.cu + v.ns; c.offx = c.offy = 0;
     c.out = v.raw_u; c.out_h = v.H; c.out_w = v.W; c.stats = v.bn_u.fwd;
     c.has_dgrad = !wide;
-    c.dg_in = v.dRaw_u; c.dg_in_h = v.H; c.dg_in_w = v.W; c.dg_out = v.dP_cat; c.dg_out_h = v.H + 2; c.dg_out_w = v.W + 2; c.dg_off = -2;
-    c.wg_dy = v.dRaw_u; c.wg_h = v.H; c.wg_w = v.W;
-    c.in16 = v.P_cat16; c.in_ld16 = v.cat_ld16; c.dg_in16 = v.dRaw_u16; c.wg_dy16 = v.dRaw_u16;
+    c.dy = v.dRaw_u; c.dy16 = v.dRaw_u16;
+    c.dg_out = v.dP_cat; c.dg_out_h = v.H + 2; c.dg_out_w = v.W + 2; c.dg_off = -2;
+    c.in16 = v.P_cat16; c.in_ld16 = v.cat_ld16;
     // 1x1: A_u -> raw_v
     ConvOp& e = v.c11;
     e.set_shapes();
     e.in = v.A_u; e.in_rows = v.H; e.in_cols = v.W; e.in_ld = v.nu; e.offx = e.offy = 0;
     e.out = v.raw_v; e.out_h = v.H; e.out_w = v.W; e.stats = v.bn_v.fwd;
     e.has_dgrad = true;
-    e.dg_in = v.dRaw_v; e.dg_in_h = v.H; e.dg_in_w = v.W; e.dg_out = v.dA_u; e.dg_out_h = v.H; e.dg_out_w = v.W; e.dg_off = 0;
-    e.wg_dy = v.dRaw_v; e.wg_h = v.H; e.wg_w = v.W;
-    e.in16 = v.A_u16; e.in_ld16 = v.nu; e.dg_in16 = v.dRaw_v16; e.wg_dy16 = v.dRaw_v16;
+    e.dy = v.dRaw_v; e.dy16 = v.dRaw_v16;
+    e.dg_out = v.dA_u; e.dg_out_h = v.H; e.dg_out_w = v.W; e.dg_off = 0;
+    e.in16 = v.A_u16; e.in_ld16 = v.nu;
     std::vector<ConvOp*> ops = {&a, &b, &c, &e};
     if (wide) {
       // skip conv 1x1 on the interior of the padded level input
@@ -959,26 +949,24 @@ static int build_plan(dip_plan* P, Arena& A) {
       k1.out = v.raw_s; k1.out_h = v.H; k1.out_w = v.W; k1.stats = v.bn_s.fwd;
       k1.has_dgrad = l > 0 || d.input_grad != 0;
       k1.dg_ld = v.Cin;
-      k1.dg_in = v.dRaw_s; k1.dg_in_h = v.H; k1.dg_in_w = v.W; k1.dg_out = v.dS; k1.dg_out_h = v.H; k1.dg_out_w = v.W; k1.dg_off = 0;
-      k1.wg_dy = v.dRaw_s; k1.wg_h = v.H; k1.wg_w = v.W;
-      k1.in16 = v.Pin16; k1.in_ld16 = v.Pin_ld16; k1.dg_in16 = v.dRaw_s16; k1.wg_dy16 = v.dRaw_s16;
+      k1.dy = v.dRaw_s; k1.dy16 = v.dRaw_s16;
+      k1.dg_out = v.dS; k1.dg_out_h = v.H; k1.dg_out_w = v.W; k1.dg_off = 0;
+      k1.in16 = v.Pin16; k1.in_ld16 = v.Pin_ld16;
       ops.push_back(&k1);
       for (ConvOp* h : {&v.up_a, &v.up_b}) {
         h->set_shapes();
         h->in = v.P_cat + h->coff; h->in_rows = v.H + 2; h->in_cols = v.W + 2; h->in_ld = 128 + CS; h->offx = h->offy = 0;
         h->out = v.raw_u; h->out_h = v.H; h->out_w = v.W; h->stats = nullptr;
         h->has_dgrad = true;
-        h->dg_in = v.dRaw_u; h->dg_in_h = v.H; h->dg_in_w = v.W;
+        h->dy = v.dRaw_u; h->dy16 = v.dRaw_u16;
         h->dg_out = v.dP_cat + h->coff; h->dg_out_h = v.H + 2; h->dg_out_w = v.W + 2; h->dg_off = -2;
-        h->wg_dy = v.dRaw_u; h->wg_h = v.H; h->wg_w = v.W;
-        h->in16 = v.P_cat16 != nullptr ? v.P_cat16 + h->coff : nullptr; h->in_ld16 = v.cat_ld16; h->dg_in16 = v.dRaw_u16; h->wg_dy16 = v.dRaw_u16;
+        h->in16 = v.P_cat16 != nullptr ? v.P_cat16 + h->coff : nullptr; h->in_ld16 = v.cat_ld16;
         ops.push_back(h);
       }
     }
     for (ConvOp* op : ops) {
       op->wp_f = op->do_fprop ? A.get<float>(op->wp_f_elems()) : nullptr;
       op->wp_d = op->has_dgrad ? A.get<float>(op->wp_d_elems()) : nullptr;
-      op->simt_ksplits = op->wg_h < 64 ? op->wg_h : 64;
       op->bf16 = bf;
       op->timer = &P->timer;
       const size_t pe = op->do_wgrad ? op->partial_elems(prec) : 0;
@@ -986,19 +974,26 @@ static int build_plan(dip_plan* P, Arena& A) {
       P->convs.push_back(op);
     }
   }
+  // split-K partials of the weight gradients.  fp32 mode: one area that every conv's wgrad writes and its own unpack entry
+  // sums right away (the tensor-core modes reserve it as well but do not use it).  Tensor-core modes: every conv's partials
+  // in their own slice of one contiguous area, summed by one launch over all entries at the end of the backward pass.
   P->partial = A.get<float>(partial_max);
-  // weight-gradient accumulators of the tensor-core path: one per conv, contiguous (a single memset per backward)
   P->n_unpack = 0;
+  for (ConvOp* op : P->convs) if (op->do_wgrad) P->n_unpack++;
   if (is_tc(prec)) {
     size_t tot = 0;
-    for (ConvOp* op : P->convs) if (op->do_wgrad) { tot += (op->wacc_elems() + 63) & ~size_t(63); P->n_unpack++; }
+    for (ConvOp* op : P->convs) if (op->do_wgrad) tot += (op->partial_elems(prec) + 63) & ~size_t(63);
     P->wacc_base = A.get<float>(tot);
     P->wacc_bytes = tot * sizeof(float);
     if (P->wacc_base != nullptr) reg("wacc", P->wacc_base, 1, 1, (int)tot, (int)tot);   // (tests NaN-fill it)
     size_t off = 0;
-    for (ConvOp* op : P->convs) if (op->do_wgrad) { op->wacc = P->wacc_base ? P->wacc_base + off : nullptr; off += (op->wacc_elems() + 63) & ~size_t(63); }
+    for (ConvOp* op : P->convs) if (op->do_wgrad) { op->partial = P->wacc_base ? P->wacc_base + off : nullptr; off += (op->partial_elems(prec) + 63) & ~size_t(63); }
   }
   P->d_unpack = A.get<UnpackEntry>(P->n_unpack > 0 ? P->n_unpack : 1);
+  if (!is_tc(prec) && !P->dry) {
+    int i = 0;
+    for (ConvOp* op : P->convs) if (op->do_wgrad) { op->partial = P->partial; op->unpack = P->d_unpack + i++; }
+  }
   P->n_pack = (int)P->convs.size();
   P->n_cvt = (int)P->bns.size() * 3 + L + 2;
   P->n_run = (int)P->bns.size();
@@ -1019,7 +1014,7 @@ static int build_plan(dip_plan* P, Arena& A) {
   for (int l = 0; l < L; ++l)
     if (P->lv[l].ZS != nullptr) DIP_CUDA(cudaMemset(P->lv[l].ZS, 0, (size_t)P->lv[l].H * P->lv[l].W * P->lv[l].nd * sizeof(float)));
   if (is_tc(prec))
-    for (ConvOp* op : P->convs) DIP_CHECK(op->build_tc(P->partial));
+    for (ConvOp* op : P->convs) DIP_CHECK(op->build_tc());
   P->pack_max = 0;
   for (ConvOp* op : P->convs) {
     const long long n = (op->do_fprop ? (long long)op->wp_f_elems() : 0) + (op->has_dgrad ? (long long)op->wp_d_elems() : 0);
@@ -1030,22 +1025,12 @@ static int build_plan(dip_plan* P, Arena& A) {
 
 static int upload_tables(dip_plan* P) {
   std::vector<PackEntry> pk;
-  for (ConvOp* op : P->convs) {
-    PackEntry e{};
-    e.w = P->params[op->p_w]; e.dst_f = op->do_fprop ? op->wp_f : nullptr; e.dst_d = op->has_dgrad ? op->wp_d : nullptr;
-    e.N = op->N; e.C = op->C; e.k = op->k; e.rot = op->rot; e.n_rows = op->Np; e.c_pad = op->c_pad; e.c_rows = op->crows;
-    e.Ctot = op->Ctot; e.coff = op->coff; e.s2 = op->dg_s2 ? 1 : 0;
-    e.bf16 = op->bf16 ? 1 : 0; e.c_pad16 = op->c_pad16; e.n_pad = op->bf16 ? op->n_pad16 : op->n_pad;
-    pk.push_back(e);
-  }
+  for (ConvOp* op : P->convs) pk.push_back(op->pack_entry(P->params[op->p_w]));
   DIP_CUDA(cudaMemcpy(P->d_pack, pk.data(), pk.size() * sizeof(PackEntry), cudaMemcpyHostToDevice));
   if (P->n_unpack > 0) {
     std::vector<UnpackEntry> up;
-    for (ConvOp* op : P->convs) {
-      if (!op->do_wgrad || op->wacc == nullptr) continue;
-      up.push_back(UnpackEntry{op->wacc, P->grads[op->p_w], op->N, op->C, op->k * op->k, op->rot, op->wg_cols(), op->Ctot, op->coff,
-                               op->wg.ksplits});
-    }
+    for (ConvOp* op : P->convs)
+      if (op->do_wgrad) up.push_back(op->unpack_entry(P->desc.precision, P->grads[op->p_w]));
     if ((int)up.size() != P->n_unpack) return fail("internal: unpack table size mismatch");
     DIP_CUDA(cudaMemcpy(P->d_unpack, up.data(), up.size() * sizeof(UnpackEntry), cudaMemcpyHostToDevice));
   }
@@ -1272,7 +1257,7 @@ static constexpr int kDeferLevel = 2;
 static int flush_deferred(dip_plan* P, int prec, cudaStream_t s) {
   if (P->deferred.empty()) return 0;
   cudaStream_t ws = fork_side(P, s);
-  for (ConvOp* op : P->deferred) DIP_CHECK(op->run_wgrad(prec, P->partial, P->grads[op->p_w], ws));
+  for (ConvOp* op : P->deferred) DIP_CHECK(op->run_wgrad(prec, ws));
   P->deferred.clear();
   return 0;
 }
@@ -1288,7 +1273,7 @@ static int conv_backward(dip_plan* P, ConvOp& op, bool dgrad, int prec, cudaStre
   }
   cudaStream_t ws = fork_side(P, s);
   if (dgrad) DIP_CHECK(op.run_dgrad(prec, s));
-  return op.run_wgrad(prec, P->partial, P->grads[op.p_w], ws);
+  return op.run_wgrad(prec, ws);
 }
 
 static int bwd_level(dip_plan* P, int l, GradSrc src_v, cudaStream_t s, int& nl) {
@@ -1297,7 +1282,7 @@ static int bwd_level(dip_plan* P, int l, GradSrc src_v, cudaStream_t s, int& nl)
   const int CS = v.ns, nd = v.nd, nu = v.nu;
   const int CC = v.cu + CS;
   const bool last = l == (int)P->lv.size() - 1;
-  const int wl = is_tc(prec) ? 1 : 2;   // tensor-core wgrads accumulate in place (no per-conv reduction launch)
+  const int wl = is_tc(prec) ? 1 : 2;   // fp32 mode: every wgrad is followed by its own split-K sum
   // 1x1 conv + BN + LReLU
   DIP_CHECK(bn_bwd(P, v.raw_v, nu, v.bn_v, 1, src_v, v.H, v.W, v.dRaw_v, nullptr, s, nl, v.dRaw_v16));
   if (l == kDeferLevel) DIP_CHECK(flush_deferred(P, prec, s));
@@ -1309,8 +1294,8 @@ static int bwd_level(dip_plan* P, int l, GradSrc src_v, cudaStream_t s, int& nl)
     cudaStream_t ws = fork_side(P, s);
     DIP_CHECK(v.up_a.run_dgrad(prec, s));
     DIP_CHECK(v.up_b.run_dgrad(prec, s));
-    DIP_CHECK(v.up_a.run_wgrad(prec, P->partial, P->grads[v.up.p_w], ws));
-    DIP_CHECK(v.up_b.run_wgrad(prec, P->partial, P->grads[v.up.p_w], ws));
+    DIP_CHECK(v.up_a.run_wgrad(prec, ws));
+    DIP_CHECK(v.up_b.run_wgrad(prec, ws));
     nl += 2 * (wl + 1);
   } else {
     DIP_CHECK(conv_backward(P, v.up, true, prec, s, l));
@@ -1333,7 +1318,7 @@ static int bwd_level(dip_plan* P, int l, GradSrc src_v, cudaStream_t s, int& nl)
   if (CS == 0) {
     // no skip branch (models/skip.py:50-53 with num_channels_skip = 0)
   } else if (CS == 128) {
-    DIP_CHECK(v.sk.run_wgrad(prec, P->partial, P->grads[v.p_skip_w], fork_side(P, ks)));
+    DIP_CHECK(v.sk.run_wgrad(prec, fork_side(P, ks)));
     nl += wl;
     if (l > 0 || P->desc.input_grad) { DIP_CHECK(v.sk.run_dgrad(prec, ks)); nl += 1; }   // dS, added to the fold of dPin by the level above
   } else {
@@ -1393,7 +1378,7 @@ static int plan_backward(dip_plan* P, const float* dout, cudaStream_t s) {
   join_skip(P, s);
   launch_k(k_cvt_table, dim3(P->n_cvt), dim3(128), 0, s, 1, P->d_cvt);
   nl += 1;
-  if (P->n_unpack > 0) {
+  if (is_tc(P->desc.precision) && P->n_unpack > 0) {   // (fp32 mode: each conv's entry ran after its wgrad)
     HBM_T(&P->timer, H_WGRAD_REDUCE, 1, 2.0 * (double)P->wacc_bytes, s,
           launch_k(k_wgrad_unpack_table, dim3(64, P->n_unpack), dim3(256), 0, s, 1, P->d_unpack));
     nl += 1;
@@ -1816,147 +1801,96 @@ int dip_plan_num_launches(const dip_plan* plan, int* fwd, int* bwd) {
 // ---------------------------------------------------------------------------------------------- single-op entry points
 size_t dip_op_scratch_bytes(void) { return (size_t)96 << 20; }
 
-// scratch layout of the single-op entry points: [fprop pack | dgrad pack | one PackEntry (64 floats) | wgrad accumulator |
-// bf16 copies of the operands (precision bf16)]
-static float* op_partial(ConvOp& op, float* scratch) {
-  return scratch + ((op.wp_f_elems() + 63) & ~size_t(63)) + ((op.wp_d_elems() + 63) & ~size_t(63)) + 64;
-}
-static int op_common(ConvOp& op, int N, int C, int k, int stride, int rot, float* scratch, const float* w, cudaStream_t s,
-                     int max_c = 160, int prec = DIP_PRECISION_TF32) {
-  if (N != 128) return fail("dip_op_conv_*: N must be 128");
-  if (C % 4 != 0 || C > max_c) return fail("dip_op_conv_*: C must be a multiple of 4 and <= " + std::to_string(max_c));
-  op.N = N; op.C = C; op.k = k; op.stride = stride; op.rot = rot;
+// Sets up one convolution that an entry point has described (shapes, tensors and which of do_fprop / has_dgrad /
+// do_wgrad it runs) in the caller's scratch area, laid out as [fprop pack | dgrad pack | PackEntry | UnpackEntry | wgrad
+// partials | bf16 copies of dY and of the input (precision bf16)].  Operands whose layout does not fit are refused before
+// anything is launched.  Then packs w, uploads the table entries, writes the bf16 copies and encodes the tensor maps.
+static int op_setup(const char* name, ConvOp& op, int prec, const float* w, float* dw, void* scratch, cudaStream_t s) {
+  DIP_CHECK(engine_init());
+  const int max_c = op.do_fprop ? 256 : 160;   // dgrad / wgrad: the register accumulators hold at most 160 columns
+  if (op.N != 128) return fail(std::string(name) + ": N must be 128");
+  if (op.C % 4 != 0 || op.C > max_c)
+    return fail(std::string(name) + ": C must be a multiple of 4 and <= " + std::to_string(max_c));
   op.bf16 = prec == DIP_PRECISION_BF16;
   op.set_shapes();
-  op.wp_f = scratch;
-  op.wp_d = scratch + ((op.wp_f_elems() + 63) & ~size_t(63));
-  if (op.bf16) {
-    // bf16 packs come from the table kernel (one entry, staged in the scratch area)
-    PackEntry e{};
-    e.w = w; e.dst_f = op.wp_f; e.dst_d = op.wp_d; e.N = N; e.C = C; e.k = k; e.rot = rot; e.n_rows = N;
-    e.c_pad = op.c_pad; e.c_rows = op.crows; e.Ctot = C; e.coff = 0; e.s2 = 0; e.bf16 = 1; e.c_pad16 = op.c_pad16;
-    PackEntry* d_e = reinterpret_cast<PackEntry*>(op_partial(op, scratch) - 64);
-    DIP_CUDA(cudaMemcpyAsync(d_e, &e, sizeof e, cudaMemcpyHostToDevice, s));
-    launch_k(k_pack_table, dim3(64, 1), dim3(256), 0, s, 1, (const PackEntry*)d_e);
-  } else {
-    launch_pack_fprop(w, N, C, k, k, rot, op.wp_f, N, op.c_pad, s);
-    launch_pack_dgrad(w, N, C, k, k, rot, op.wp_d, op.crows, 128, s);
+  const bool pack = op.do_fprop || op.has_dgrad;
+  const bool cast_dy = op.bf16 && (op.has_dgrad || op.do_wgrad), cast_in = op.bf16 && (op.do_fprop || op.do_wgrad);
+  if (cast_in) op.in_ld16 = round_up(op.in_ld, 8);
+  Arena A{(uint8_t*)scratch};
+  op.wp_f = op.do_fprop ? A.get<float>(op.wp_f_elems()) : nullptr;
+  op.wp_d = op.has_dgrad ? A.get<float>(op.wp_d_elems()) : nullptr;
+  PackEntry* d_pack = pack ? A.get<PackEntry>(1) : nullptr;
+  UnpackEntry* d_unpack = op.do_wgrad ? A.get<UnpackEntry>(1) : nullptr;
+  op.partial = op.do_wgrad ? A.get<float>(op.partial_elems(prec)) : nullptr;
+  const long long dy_px = (long long)op.out_h * op.out_w, in_px = (long long)op.in_rows * op.in_cols;
+  uint16_t* dy16 = cast_dy ? A.get<uint16_t>(dy_px * op.N) : nullptr;
+  uint16_t* in16 = cast_in ? A.get<uint16_t>(in_px * op.in_ld16) : nullptr;
+  if (A.off > dip_op_scratch_bytes())
+    return fail(std::string(name) + ": the operands need " + std::to_string((A.off + (1 << 20) - 1) >> 20) +
+                " MB of scratch, more than dip_op_scratch_bytes() = " + std::to_string(dip_op_scratch_bytes() >> 20) + " MB");
+  if (pack) {
+    const PackEntry e = op.pack_entry(w);
+    DIP_CUDA(cudaMemcpyAsync(d_pack, &e, sizeof e, cudaMemcpyHostToDevice, s));
+    launch_k(k_pack_table, dim3(64, 1), dim3(256), 0, s, 1, (const PackEntry*)d_pack);
   }
+  if (op.do_wgrad) {
+    const UnpackEntry e = op.unpack_entry(prec, dw);
+    DIP_CUDA(cudaMemcpyAsync(d_unpack, &e, sizeof e, cudaMemcpyHostToDevice, s));
+    op.unpack = d_unpack;
+  }
+  if (cast_dy) launch_cast_bf16(op.dy, op.N, op.N, dy_px, Twin{dy16, op.N}, s);
+  if (cast_in) launch_cast_bf16(op.in, op.in_ld, op.in_ld, in_px, Twin{in16, op.in_ld16}, s);
+  op.dy16 = dy16; op.in16 = in16;
   DIP_CUDA(cudaGetLastError());
-  return 0;
-}
-// precision bf16: bf16 copy of an NHWC fp32 operand [npix][ld] in the scratch area behind *area (advanced)
-static const uint16_t* op_cast(const void* x, int ld, long long npix, uint16_t** area, int* ld16, cudaStream_t s) {
-  *ld16 = round_up(ld, 8);
-  uint16_t* dst = *area;
-  *area += ((size_t)npix * *ld16 + 127) & ~size_t(127);
-  launch_cast_bf16((const float*)x, ld, ld, npix, Twin{dst, *ld16}, s);
-  return dst;
-}
-static uint16_t* op_cast_area(ConvOp& op, float* partial) {
-  return reinterpret_cast<uint16_t*>(partial + ((op.wacc_elems() + 63) & ~size_t(63)));
+  return is_tc(prec) ? op.build_tc() : 0;
 }
 
 int dip_op_conv_fprop(const void* a, int a_h, int a_w, int a_c, const void* w, const void* bias, int N, int C, int k, int stride,
                       int offx, int offy, int rot, void* d, int d_h, int d_w, double* stats, int precision, void* scratch,
                       dip_stream_t stream) {
-  DIP_CHECK(engine_init());
   cudaStream_t s = (cudaStream_t)stream;
   ConvOp op;
-  DIP_CHECK(op_common(op, N, C, k, stride, rot, (float*)scratch, (const float*)w, s, 256, precision));
+  op.N = N; op.C = C; op.k = k; op.stride = stride; op.rot = rot;
+  op.do_fprop = true; op.has_dgrad = false; op.do_wgrad = false;
   op.in = (const float*)a; op.in_rows = a_h; op.in_cols = a_w; op.in_ld = a_c; op.offx = offx; op.offy = offy;
   op.out = (float*)d; op.out_h = d_h; op.out_w = d_w; op.stats = stats;
-  op.has_dgrad = false;
-  op.wg_dy = (const float*)d; op.wg_h = d_h; op.wg_w = d_w;  // placeholders so that build_tc can encode maps
-  if (op.bf16) {
-    uint16_t* area = op_cast_area(op, op_partial(op, (float*)scratch));
-    op.in16 = op_cast(a, a_c, (long long)a_h * a_w, &area, &op.in_ld16, s);
-    op.do_wgrad = false;
-  }
-  if (is_tc(precision)) DIP_CHECK(op.build_tc(op_partial(op, (float*)scratch)));
+  DIP_CHECK(op_setup("dip_op_conv_fprop", op, precision, (const float*)w, nullptr, scratch, s));
   return op.run_fprop(precision, (const float*)bias, s);
 }
 int dip_op_conv_dgrad(const void* dy, int dy_h, int dy_w, const void* w, int N, int C, int k, int rot, void* dx, int dx_h, int dx_w,
                       int precision, void* scratch, dip_stream_t stream) {
-  DIP_CHECK(engine_init());
   cudaStream_t s = (cudaStream_t)stream;
   ConvOp op;
-  DIP_CHECK(op_common(op, N, C, k, 1, rot, (float*)scratch, (const float*)w, s, 160, precision));
-  // fprop/wgrad placeholders (valid maps over the same buffers; not launched)
-  op.in = (const float*)dx; op.in_rows = dx_h; op.in_cols = dx_w; op.in_ld = C; op.out = (float*)const_cast<void*>(dy);
-  op.out_h = dy_h; op.out_w = dy_w; op.wg_dy = (const float*)dy; op.wg_h = dy_h; op.wg_w = dy_w;
-  op.has_dgrad = true;
-  op.dg_in = (const float*)dy; op.dg_in_h = dy_h; op.dg_in_w = dy_w;
+  op.N = N; op.C = C; op.k = k; op.rot = rot;
+  op.do_fprop = false; op.has_dgrad = true; op.do_wgrad = false;
+  op.dy = (const float*)dy; op.out_h = dy_h; op.out_w = dy_w;
   op.dg_out = (float*)dx; op.dg_out_h = dx_h; op.dg_out_w = dx_w; op.dg_off = -(k - 1);
-  if (op.bf16) {
-    uint16_t* area = op_cast_area(op, op_partial(op, (float*)scratch));
-    int ld16 = 0;
-    op.dg_in16 = op_cast(dy, 128, (long long)dy_h * dy_w, &area, &ld16, s);
-    op.do_fprop = false; op.do_wgrad = false;
-  }
-  if (is_tc(precision)) DIP_CHECK(op.build_tc(op_partial(op, (float*)scratch)));
+  DIP_CHECK(op_setup("dip_op_conv_dgrad", op, precision, (const float*)w, nullptr, scratch, s));
   return op.run_dgrad(precision, s);
 }
 int dip_op_conv_dgrad_s2(const void* dy, int dy_h, int dy_w, const void* w, int N, int C, int rot, void* dx, int precision,
                          void* scratch, dip_stream_t stream) {
-  DIP_CHECK(engine_init());
   if (!is_tc(precision)) return fail("dip_op_conv_dgrad_s2: tensor-core path only (the exact-fp32 mode zero-stuffs)");
   cudaStream_t s = (cudaStream_t)stream;
   ConvOp op;
-  if (N != 128) return fail("dip_op_conv_dgrad_s2: N must be 128");
-  if (C % 4 != 0 || C > 160) return fail("dip_op_conv_dgrad_s2: C must be a multiple of 4 and <= 160");
   op.N = N; op.C = C; op.k = 3; op.stride = 2; op.rot = rot;
-  op.bf16 = precision == DIP_PRECISION_BF16;
-  op.set_shapes();
-  op.wp_f = (float*)scratch;
-  op.wp_d = (float*)scratch + ((op.wp_f_elems() + 63) & ~size_t(63));
-  // one-entry pack table in the scratch area behind the packed weights
-  PackEntry e{};
-  e.w = (const float*)w; e.dst_f = nullptr; e.dst_d = op.wp_d; e.N = N; e.C = C; e.k = 3; e.rot = rot; e.n_rows = N;
-  e.c_pad = op.c_pad; e.c_rows = op.crows; e.Ctot = C; e.coff = 0; e.s2 = 1; e.bf16 = op.bf16 ? 1 : 0; e.c_pad16 = op.c_pad16;
-  PackEntry* d_e = reinterpret_cast<PackEntry*>(op_partial(op, (float*)scratch) - 64);
-  DIP_CUDA(cudaMemcpyAsync(d_e, &e, sizeof e, cudaMemcpyHostToDevice, s));
-  launch_k(k_pack_table, dim3(64, 1), dim3(256), 0, s, 1, (const PackEntry*)d_e);
-  op.do_fprop = false; op.do_wgrad = false;
-  op.has_dgrad = true; op.dg_s2 = true;
-  op.dg_in = (const float*)dy; op.dg_in_h = dy_h; op.dg_in_w = dy_w;
+  op.do_fprop = false; op.has_dgrad = true; op.do_wgrad = false;
+  op.dg_s2 = true;
+  op.dy = (const float*)dy; op.out_h = dy_h; op.out_w = dy_w;
   op.dg_out = (float*)dx; op.dg_out_h = 2 * dy_h + 2; op.dg_out_w = 2 * dy_w + 2; op.dg_off = -2;
-  if (op.bf16) {
-    uint16_t* area = op_cast_area(op, op_partial(op, (float*)scratch));
-    int ld16 = 0;
-    op.dg_in16 = op_cast(dy, 128, (long long)dy_h * dy_w, &area, &ld16, s);
-  }
-  DIP_CHECK(op.build_tc(nullptr));
+  DIP_CHECK(op_setup("dip_op_conv_dgrad_s2", op, precision, (const float*)w, nullptr, scratch, s));
   return op.run_dgrad(precision, s);
 }
 int dip_op_conv_wgrad(const void* dy, int dy_h, int dy_w, const void* a, int a_h, int a_w, int a_c, int N, int C, int k, int stride,
                       int offx, int offy, int rot, void* dw, int precision, void* scratch, dip_stream_t stream) {
-  DIP_CHECK(engine_init());
   cudaStream_t s = (cudaStream_t)stream;
   ConvOp op;
-  // weights are not needed for wgrad; pack from dw is skipped
-  if (N != 128) return fail("dip_op_conv_wgrad: N must be 128");
   op.N = N; op.C = C; op.k = k; op.stride = stride; op.rot = rot;
-  op.bf16 = precision == DIP_PRECISION_BF16;
-  op.set_shapes();
-  op.wp_f = (float*)scratch;
-  op.wp_d = nullptr;
+  op.do_fprop = false; op.has_dgrad = false; op.do_wgrad = true;
   op.in = (const float*)a; op.in_rows = a_h; op.in_cols = a_w; op.in_ld = a_c; op.offx = offx; op.offy = offy;
-  op.out = (float*)const_cast<void*>(dy); op.out_h = dy_h; op.out_w = dy_w;
-  op.has_dgrad = false;
-  op.wg_dy = (const float*)dy; op.wg_h = dy_h; op.wg_w = dy_w;
-  op.simt_ksplits = dy_h < 64 ? dy_h : 64;
-  float* partial = (float*)scratch + ((op.wp_f_elems() + 63) & ~size_t(63));
-  if (op.bf16) {
-    uint16_t* area = op_cast_area(op, partial);
-    int ld16 = 0;
-    op.wg_dy16 = op_cast(dy, 128, (long long)dy_h * dy_w, &area, &ld16, s);
-    op.in16 = op_cast(a, a_c, (long long)a_h * a_w, &area, &op.in_ld16, s);
-    op.do_fprop = false;
-    if ((uint8_t*)area > (uint8_t*)scratch + dip_op_scratch_bytes()) return fail("dip_op_conv_wgrad: operands too large for the scratch area (bf16 copies)");
-  }
-  if (is_tc(precision)) DIP_CHECK(op.build_tc(partial));
-  return op.run_wgrad(precision, partial, (float*)dw, s);
+  op.dy = (const float*)dy; op.out_h = dy_h; op.out_w = dy_w;
+  DIP_CHECK(op_setup("dip_op_conv_wgrad", op, precision, nullptr, (float*)dw, scratch, s));
+  return op.run_wgrad(precision, s);
 }
 
 }  // extern "C"

@@ -229,20 +229,6 @@ cudaError_t launch_down_fwd(const float* x, int C, int H, int W, const float* ke
 cudaError_t launch_down_bwd(const float* dy, int C, int H, int W, const float* kern, int K, int f, int pad, float* dx,
                             cudaStream_t s);
 
-// weight repacking ---------------------------------------------------------------------------------
-// torch OIHW [N][C][kh][kw]  ->  fprop pack [tap][n_rows][c_pad] (K-major), channel rotation c_t = (c + rot) % C
-void launch_pack_fprop(const float* w, int N, int C, int kh, int kw, int rot, float* dst, int n_rows, int c_pad,
-                       cudaStream_t s);
-// -> dgrad pack [tap'][c_rows][n_pad] with tap' = flipped tap, rows = input channel (rotated), cols = out channel
-void launch_pack_dgrad(const float* w, int N, int C, int kh, int kw, int rot, float* dst, int c_rows, int n_pad,
-                       cudaStream_t s);
-// split-K partials [ksplits][tap][128][c_pad] -> OIHW gradient [N][C][kh][kw]
-//   c_pad: row stride of the partials (a multiple of 4, >= C; the tensor-core path passes its accumulator columns)
-//   dw has Ctot input channels; the partials cover engine channels [coff, coff + C): torch channel (c + coff + rot) % Ctot
-//   (Ctot = 0: Ctot = C)
-void launch_wgrad_reduce(const float* partial, int ksplits, int N, int C, int kh, int kw, int rot, int c_pad,
-                         float* dw, cudaStream_t s, int Ctot = 0, int coff = 0);
-
 // Adam ---------------------------------------------------------------------------------------------
 struct AdamTable {
   float* const* p;

@@ -1509,91 +1509,6 @@ __global__ void k_advance(int* it) {
   pdl_enter(); it[0] += 1; it[1] += 1; }  // {global Adam step, iteration index of this call}
 void launch_advance(int* it_dev, cudaStream_t s) { launch_k(k_advance, dim3(1), dim3(1), 0, s, 1, it_dev); }
 
-// ------------------------------------------------------------------------------------------------ weight packing
-__global__ void k_pack_fprop(const float* __restrict__ w, int N, int C, int kh, int kw, int rot, float* __restrict__ dst,
-                             int n_rows, int c_pad) {
-  pdl_enter();
-  const long long total = static_cast<long long>(kh) * kw * n_rows * c_pad;
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int c = static_cast<int>(i % c_pad);
-    const int n = static_cast<int>((i / c_pad) % n_rows);
-    const int tap = static_cast<int>(i / (static_cast<long long>(c_pad) * n_rows));
-    float val = 0.f;
-    if (n < N && c < C) val = w[(static_cast<long long>(n) * C + (c + rot) % C) * (kh * kw) + tap];
-    dst[i] = val;
-  }
-}
-void launch_pack_fprop(const float* w, int N, int C, int kh, int kw, int rot, float* dst, int n_rows, int c_pad,
-                       cudaStream_t s) {
-  const long long total = static_cast<long long>(kh) * kw * n_rows * c_pad;
-  launch_k(k_pack_fprop, dim3(static_cast<int>((total + 255) / 256)), dim3(256), 0, s, 1, w, N, C, kh, kw, rot, dst, n_rows, c_pad);
-}
-__global__ void k_pack_dgrad(const float* __restrict__ w, int N, int C, int kh, int kw, int rot, float* __restrict__ dst,
-                             int c_rows, int n_pad) {
-  pdl_enter();
-  const long long total = static_cast<long long>(kh) * kw * c_rows * n_pad;
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int n = static_cast<int>(i % n_pad);
-    const int c = static_cast<int>((i / n_pad) % c_rows);
-    const int tapf = static_cast<int>(i / (static_cast<long long>(n_pad) * c_rows));
-    const int tap = kh * kw - 1 - tapf;  // (kh-1-r', kw-1-s')
-    float val = 0.f;
-    if (n < N && c < C) val = w[(static_cast<long long>(n) * C + (c + rot) % C) * (kh * kw) + tap];
-    dst[i] = val;
-  }
-}
-void launch_pack_dgrad(const float* w, int N, int C, int kh, int kw, int rot, float* dst, int c_rows, int n_pad,
-                       cudaStream_t s) {
-  const long long total = static_cast<long long>(kh) * kw * c_rows * n_pad;
-  launch_k(k_pack_dgrad, dim3(static_cast<int>((total + 255) / 256)), dim3(256), 0, s, 1, w, N, C, kh, kw, rot, dst, c_rows, n_pad);
-}
-
-// Split-K reduction.  Block = 32 float4 columns x 8 split-parts: a warp reads 512 contiguous bytes of one split;
-// the 8 parts are folded through shared memory (deterministic order), then scattered to the OIHW gradient.
-__global__ void __launch_bounds__(256) k_wgrad_reduce(const float* __restrict__ partial, int ksplits, int N, int C, int taps,
-                                                      int rot, int c_pad, float* __restrict__ dw, int Ctot, int coff) {
-  pdl_enter();
-  __shared__ float4 sm[8][32];
-  const int e = threadIdx.x & 31, part = threadIdx.x >> 5;
-  const int c4n = c_pad / 4;
-  const int total4 = taps * 128 * c4n;
-  const int idx = blockIdx.x * 32 + e;  // (tap, n, c4)
-  float4 s = f4zero();
-  if (idx < total4) {
-    const size_t split_stride = static_cast<size_t>(taps) * 128 * c_pad;
-    const float* src = partial + static_cast<size_t>(idx) * 4;
-    int k = part;
-    for (; k + 8 < ksplits; k += 16) {
-      const float4 a = ld4(src + k * split_stride);
-      const float4 b = ld4(src + (k + 8) * split_stride);
-      s = f4add(s, f4add(a, b));
-    }
-    for (; k < ksplits; k += 8) s = f4add(s, ld4(src + k * split_stride));
-  }
-  sm[part][e] = s;
-  __syncthreads();
-  if (part == 0 && idx < total4) {
-#pragma unroll
-    for (int q = 1; q < 8; ++q) s = f4add(s, sm[q][e]);
-    const int c4 = idx % c4n, n = (idx / c4n) % 128, tap = idx / (c4n * 128);
-    const float sv[4] = {s.x, s.y, s.z, s.w};
-    if (n < N) {
-      for (int q = 0; q < 4; ++q) {
-        const int c = 4 * c4 + q;
-        if (c < C) dw[(static_cast<size_t>(n) * Ctot + (c + coff + rot) % Ctot) * taps + tap] = sv[q];
-      }
-    }
-  }
-}
-void launch_wgrad_reduce(const float* partial, int ksplits, int N, int C, int kh, int kw, int rot, int c_pad,
-                         float* dw, cudaStream_t s, int Ctot, int coff) {
-  const int total4 = kh * kw * 128 * (c_pad / 4);
-  launch_k(k_wgrad_reduce, dim3((total4 + 31) / 32), dim3(256), 0, s, 1, partial, ksplits, N, C, kh * kw, rot, c_pad, dw,
-           Ctot > 0 ? Ctot : C, coff);
-}
-
 // ------------------------------------------------------------------------------------------------ Adam
 // Arithmetic order follows torch.optim.Adam (single-tensor path): m = lerp(m, g, 1-b1); v = v*b2 + (1-b2) g^2;
 // p -= (lr/bc1) * m / (sqrt(v)/sqrt(bc2) + eps).  Bias corrections are evaluated in fp64 on the device so that the

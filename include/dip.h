@@ -155,7 +155,9 @@ int dip_plan_get_timing_records(dip_plan* plan, int max_records, int* cls, doubl
 /* ---- single-op entry points (same kernels as the plan; used by the per-kernel parity tests).
  * Convolution of an NHWC fp32 tensor a[a_h][a_w][a_c] with torch OIHW weights w[N][C][k][k]:
  *   d[y][x][n] = bias[n] + sum a[y*stride+offy+r][x*stride+offx+s][c] * w[n][(c+rot)%C][r][s], out-of-range reads = 0.
- * scratch: device buffer of at least dip_op_scratch_bytes(). stats (nullable): 2*N fp64
+ * scratch: device buffer of at least dip_op_scratch_bytes(); it holds the packed weights, the weight-gradient partials
+ * and, in precision bf16, bf16 copies of the operands.  Operands that do not fit return an error naming the scratch,
+ * and nothing is launched. stats (nullable): 2*N fp64
  * accumulators (sum, sum^2), accumulated: element i lives at stats[16*i] (one accumulator per 128-byte line, so the
  * fp64 atomics of neighbouring channels never share an L2 line); the buffer holds 2*N*16 doubles. */
 size_t dip_op_scratch_bytes(void);

@@ -127,3 +127,40 @@ def test_dgrad_stride2_phases(case, prec):
     got = dx.permute(2, 0, 1).cpu()
     assert rel_err(got[:, :2 * h + 1, :2 * w_ + 1], ref) < TOL[prec]
     assert got[:, 2 * h + 1, :].abs().max() == 0 and got[:, :, 2 * w_ + 1].abs().max() == 0
+
+
+@pytest.mark.parametrize("op", ["fprop", "dgrad", "dgrad_s2", "wgrad"])
+def test_bf16_operands_too_large_for_the_scratch_are_refused(op):
+    """In bf16 the single-op entry points copy their operands to bf16 inside the caller's scratch area.  A 1024 x 1024 x
+    128 operand (256 MB as bf16, more than dip_op_scratch_bytes()) is refused with an error that names the scratch,
+    before anything is launched: the caller's NaN-filled output is left as it was."""
+    import dip_engine as de
+    L = de.lib()
+    h, w_ = 1024, 1024
+    big = torch.zeros(h, w_, 128, device="cuda")   # NHWC: the input of the fprop, dY of the other three
+    assert h * w_ * 128 * 2 > L.dip_op_scratch_bytes()
+    nan = float("nan")
+    scratch, s = de._ptr(de._get_scratch(big.device)), de._stream()
+    if op == "fprop":
+        w, b = torch.zeros(128, 128, 1, 1, device="cuda"), torch.zeros(128, device="cuda")
+        out = torch.full((h, w_, 128), nan, device="cuda")
+        rc = L.dip_op_conv_fprop(de._ptr(big), h, w_, 128, de._ptr(w), de._ptr(b), 128, 128, 1, 1, 0, 0, 0, de._ptr(out), h,
+                                 w_, None, de.PRECISION_BF16, scratch, s)
+    elif op == "dgrad":
+        w = torch.zeros(128, 4, 3, 3, device="cuda")
+        out = torch.full((h + 2, w_ + 2, 4), nan, device="cuda")
+        rc = L.dip_op_conv_dgrad(de._ptr(big), h, w_, de._ptr(w), 128, 4, 3, 0, de._ptr(out), h + 2, w_ + 2,
+                                 de.PRECISION_BF16, scratch, s)
+    elif op == "dgrad_s2":
+        w = torch.zeros(128, 4, 3, 3, device="cuda")
+        out = torch.full((2 * h + 2, 2 * w_ + 2, 4), nan, device="cuda")
+        rc = L.dip_op_conv_dgrad_s2(de._ptr(big), h, w_, de._ptr(w), 128, 4, 0, de._ptr(out), de.PRECISION_BF16, scratch, s)
+    else:
+        a = torch.zeros(h, w_, 4, device="cuda")
+        out = torch.full((128, 4, 1, 1), nan, device="cuda")
+        rc = L.dip_op_conv_wgrad(de._ptr(big), h, w_, de._ptr(a), h, w_, 4, 128, 4, 1, 1, 0, 0, 0, de._ptr(out),
+                                 de.PRECISION_BF16, scratch, s)
+    with pytest.raises(RuntimeError, match="scratch"):
+        de.check(rc)
+    torch.cuda.synchronize()
+    assert torch.isnan(out).all()

@@ -81,7 +81,7 @@ CONFIGS = [
     ("denoise_cs4_tf32", "denoise", lambda: E.cfg_of("cs4"), 128, 128, "tf32"),
     # bf16 weight twins repacked every iteration
     ("denoise_cs4_bf16", "denoise", lambda: E.cfg_of("cs4"), 128, 128, "bf16"),
-    # the SIMT convolutions and k_wgrad_reduce
+    # the SIMT convolutions, each weight gradient summed by k_wgrad_unpack_table on its own entry
     ("denoise_cs4_fp32", "denoise", lambda: E.cfg_of("cs4"), 64, 96, "fp32"),
     # the two-part up-conv weight gradient (up_a / up_b) into one tensor; the masked loss
     ("inpaint_cs128_tf32", "inpaint", lambda: E.cfg_of("cs128"), 128, 192, "tf32"),
