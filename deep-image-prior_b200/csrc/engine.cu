@@ -137,8 +137,8 @@ static void pick_tile(int w, int h, int* bw, int* bh) {
   }
 }
 static int round_up(int x, int m) { return (x + m - 1) / m * m; }
-// ------------------------------------------------------------------------------------------------ kernel timing
-// Optional CUDA-event brackets around every tensor-core launch (bench.py roofline: algorithmic FLOPs / device time).
+// ------------------------------------------------------------------------------------------------ enqueue recorder
+// Optional CUDA-event brackets around the timed launches (bench.py roofline: algorithmic FLOPs / device time).
 struct Timer {
   bool on = false;
   std::vector<cudaEvent_t> pool;
@@ -152,23 +152,34 @@ struct Timer {
   }
   void reset() { used = 0; recs.clear(); }
 };
-struct TimeScope {
-  Timer* t; int cls; double flops; size_t e0 = 0; cudaStream_t s;
-  TimeScope(Timer* t_, int cls_, double flops_, cudaStream_t s_) : t(t_ && t_->on ? t_ : nullptr), cls(cls_), flops(flops_), s(s_) {
-    if (t) e0 = t->get(s);
-  }
-  ~TimeScope() { if (t) { size_t e1 = t->get(s); t->recs.push_back({cls, flops, e0, e1}); } }
+// Every operation a pass enqueues (kernel launch, memset, copy) goes through one Recorder: it counts them, and brackets
+// those with a timing class when timing is on.
+struct Recorder {
+  Timer* timer = nullptr;
+  int n = 0;   // operations enqueued since the pass reset it
 };
-
-// HBM-bound launches are recorded as class 16 + 8 * kernel id + sub-kind; the "flops" field of the record then carries the
-// launch's ALGORITHMIC bytes (unique elements its contract reads + writes, x 4 B; SURVEY.md 8d) -- bench.py's HBM rooflines.
+// Timing classes: 0 fprop, 1 dgrad, 2 wgrad (the record carries the algorithmic FLOPs); HBM-bound launches are class
+// 16 + 8 * kernel id + sub-kind, and the record then carries the launch's ALGORITHMIC bytes (unique elements its contract
+// reads + writes, x 4 B; SURVEY.md 8d) -- bench.py's HBM rooflines.  kUntimed: counted only.
 enum HbmId { H_INPUT_PAD = 0, H_NOISE, H_SKINNY_FWD, H_BN_ACT_WRITE, H_BN_ACT_HEAD, H_CAT_STATS, H_CAT_WRITE, H_BN_BWD_REDUCE,
              H_BN_BWD_APPLY, H_CAT_BWD_REDUCE, H_CAT_BWD_APPLY, H_UPADJ, H_SKINNY_BWD, H_MSE, H_ADAM, H_HEAD_DLOGIT, H_DOWN_FWD,
              H_DOWN_BWD, H_PACK, H_WGRAD_REDUCE };
-#define HBM_T(timer, id, sub, bytes, s, stmt)                                              \
-  do {                                                                                     \
-    TimeScope _ts((timer), 16 + 8 * (int)(id) + (int)(sub), (double)(bytes), (s));         \
-    stmt;                                                                                  \
+static constexpr int kUntimed = -1;
+static int hbm(HbmId id, int sub) { return 16 + 8 * (int)id + sub; }
+struct EnqScope {
+  Timer* t; int cls; double flops; size_t e0 = 0; cudaStream_t s;
+  EnqScope(Recorder* r, int cls_, double flops_, cudaStream_t s_)
+      : t(r != nullptr && cls_ != kUntimed && r->timer->on ? r->timer : nullptr), cls(cls_), flops(flops_), s(s_) {
+    if (r != nullptr) r->n++;
+    if (t) e0 = t->get(s);
+  }
+  ~EnqScope() { if (t) { size_t e1 = t->get(s); t->recs.push_back({cls, flops, e0, e1}); } }
+};
+// enqueues `stmt` (one operation) through the recorder `rec` (nullptr: neither counted nor timed)
+#define ENQ(rec, cls, flops, s, stmt)                                 \
+  do {                                                                \
+    EnqScope _es((rec), (cls), (double)(flops), (s));                 \
+    stmt;                                                             \
   } while (0)
 
 // ------------------------------------------------------------------------------------------------ weight pack and split-K sum
@@ -246,7 +257,7 @@ static void fit_stages(TcConvParams& p) {
   while (tc_conv_smem_bytes(p) > 232448 && p.stages > 2) p.stages--;
 }
 struct ConvOp {
-  Timer* timer = nullptr;
+  Recorder* rec = nullptr;   // the plan's; the single-op entry points count and time nothing
   double alg_flops() const { return 2.0 * out_h * out_w * (double)N * C * k * k; }
   // N output channels (a multiple of 8, <= 128: num_channels_down / num_channels_up of the level), C input channels
   int N = 128, C = 0, k = 1, stride = 1, rot = 0;
@@ -425,24 +436,22 @@ struct ConvOp {
     if (is_tc(prec)) {
       TcConvParams p = fp;
       p.bias = bias;
-      TimeScope ts(timer, 0, alg_flops(), s);
-      DIP_CUDA(tc_conv_launch(p, g_num_sms, s));
+      ENQ(rec, 0, alg_flops(), s, DIP_CUDA(tc_conv_launch(p, g_num_sms, s)));
     } else {
       SimtConvArgs a{};
       a.A = in; a.a_h = in_rows; a.a_w = in_cols; a.a_ld = in_ld; a.a_c = C;
       a.Wp = wp_f; a.n_rows = Np; a.c_pad = c_pad;
       a.D = out; a.d_h = out_h; a.d_w = out_w; a.d_ld = N; a.d_c = N;
       a.kh = a.kw = k; a.stride = stride; a.offx = offx; a.offy = offy; a.bias = bias;
-      launch_simt_conv(a, s);
-      if (stats != nullptr) launch_channel_stats(out, N, N, out_h * out_w, stats, s);
+      ENQ(rec, kUntimed, 0, s, launch_simt_conv(a, s));
+      if (stats != nullptr) ENQ(rec, kUntimed, 0, s, launch_channel_stats(out, N, N, out_h * out_w, stats, s));
       DIP_CUDA(cudaGetLastError());
     }
     return 0;
   }
   int run_dgrad(int prec, cudaStream_t s) {
     if (is_tc(prec)) {
-      TimeScope ts(timer, 1, alg_flops(), s);
-      DIP_CUDA(tc_conv_launch(dg, g_num_sms, s));
+      ENQ(rec, 1, alg_flops(), s, DIP_CUDA(tc_conv_launch(dg, g_num_sms, s)));
     } else {
       SimtConvArgs a{};
       a.A = zs != nullptr ? zs : dy; a.a_h = zs != nullptr ? 2 * out_h : out_h; a.a_w = zs != nullptr ? 2 * out_w : out_w;
@@ -450,7 +459,7 @@ struct ConvOp {
       a.Wp = wp_d; a.n_rows = crows; a.c_pad = n_pad;
       a.D = dg_out; a.d_h = dg_out_h; a.d_w = dg_out_w; a.d_ld = dg_ld; a.d_c = C;
       a.kh = a.kw = k; a.stride = 1; a.offx = a.offy = dg_off; a.bias = nullptr;
-      launch_simt_conv(a, s);
+      ENQ(rec, kUntimed, 0, s, launch_simt_conv(a, s));
       DIP_CUDA(cudaGetLastError());
     }
     return 0;
@@ -461,19 +470,18 @@ struct ConvOp {
     static const bool dbg_skip = getenv("DIP_DBG_SKIP_WGRAD") != nullptr;   // timing diagnostic only: gradients are wrong
     if (dbg_skip) return 0;
     if (is_tc(prec)) {
-      TimeScope ts(timer, 2, alg_flops(), s);
-      DIP_CUDA(tc_wgrad_launch(wg, s));
+      ENQ(rec, 2, alg_flops(), s, DIP_CUDA(tc_wgrad_launch(wg, s)));
     } else {
       SimtWgradArgs a{};
       a.dY = dy; a.h = out_h; a.w = out_w; a.dy_ld = N; a.n = N;
       a.X = in; a.x_h = in_rows; a.x_w = in_cols; a.x_ld = in_ld; a.x_c = C;
       a.kh = a.kw = k; a.stride = stride; a.offx = offx; a.offy = offy;
       a.partial = partial; a.c_pad = c_pad; a.ksplits = simt_ksplits();
-      launch_simt_wgrad(a, s);
+      ENQ(rec, kUntimed, 0, s, launch_simt_wgrad(a, s));
     }
     if (unpack != nullptr)
-      HBM_T(timer, H_WGRAD_REDUCE, 0, ((double)part_ks(prec) + 1.0) * k * k * 128.0 * part_cols(prec) * sizeof(float), s,
-            launch_k(k_wgrad_unpack_table, dim3(64, 1), dim3(256), 0, s, 1, unpack));
+      ENQ(rec, hbm(H_WGRAD_REDUCE, 0), ((double)part_ks(prec) + 1.0) * k * k * 128.0 * part_cols(prec) * sizeof(float), s,
+          launch_k(k_wgrad_unpack_table, dim3(64, 1), dim3(256), 0, s, 1, unpack));
     DIP_CUDA(cudaGetLastError());
     return 0;
   }
@@ -640,6 +648,7 @@ struct dip_plan {
   int nbt_is_float = 0;
   int launches_fwd = 0, launches_bwd = 0;
   Timer timer;
+  Recorder rec{&timer};   // plan_forward (with the runner's early repack) and plan_backward
 };
 
 namespace dip {
@@ -789,101 +798,74 @@ static int build_plan(dip_plan* P, Arena& A) {
     P->db_head = b;
     P->db_scratch = b ? b + 4 * kAccS : nullptr;
   }
-  // ---- activations
+  // ---- activations.  One statement allocates each level buffer [rows][cols][ld] (c valid channels) and registers it as
+  // L<l>.<name> (dip_plan_buffer), under the condition on which a launch of the plan writes it.
   auto reg = [&](const std::string& name, void* p, int rows, int cols, int ld, int c) { P->bufs[name] = BufInfo{p, rows, cols, ld, c}; };
   for (int l = 0; l < L; ++l) {
     Level& v = P->lv[l];
     const std::string pf = "L" + std::to_string(l) + ".";
-    const size_t HW = (size_t)v.H * v.W, hw = (size_t)v.h * v.w;
-    const size_t HWp = (size_t)(v.H + 2) * (v.W + 2), hwp = (size_t)(v.h + 2) * (v.w + 2);
+    auto f32 = [&](const char* name, int rows, int cols, int ld, int c) {
+      float* p = A.get<float>((size_t)rows * cols * ld);
+      reg(pf + name, p, rows, cols, ld, c);
+      return p;
+    };
+    auto b16 = [&](const char* name, int rows, int cols, int ld, int c) {   // bf16 twin (names end in "16")
+      uint16_t* p = A.get<uint16_t>((size_t)rows * cols * ld);
+      reg(pf + name, p, rows, cols, ld, c);
+      return p;
+    };
     const bool last = l == L - 1;
     const int CS = v.ns, nd = v.nd, nu = v.nu, CC = v.cu + v.ns;
-    if (l == 0) v.Pin = A.get<float>(HWp * v.Cin); else v.Pin = P->lv[l - 1].P_d2;
-    v.raw_s = A.get<float>(HW * CS);
-    v.raw_d1 = A.get<float>(hw * nd);
-    v.P_d1 = A.get<float>(hwp * nd);
-    v.raw_d2 = A.get<float>(hw * nd);
-    v.P_d2 = A.get<float>(last ? hw * nd : hwp * nd);
-    v.P_cat = A.get<float>(HWp * CC);
-    v.raw_u = A.get<float>(HW * nu);
-    v.A_u = A.get<float>(HW * nu);
-    v.raw_v = A.get<float>(HW * nu);
-    v.U = (l > 0 || nu != 128) ? A.get<float>(HW * nu) : nullptr;  // a 128-deep level 0 feeds the fused RGB head instead
-    v.dRaw_v = A.get<float>(HW * nu);
-    v.dA_u = A.get<float>(HW * nu);
-    v.dRaw_u = A.get<float>(HW * nu);
-    v.dP_cat = A.get<float>(HWp * CC);
-    v.dCat = A.get<float>(HW * CC);
-    v.dRaw_s = A.get<float>(HW * CS);
-    v.dUp = A.get<float>(hw * v.cu);
-    v.dRaw_d2 = A.get<float>(hw * nd);
-    v.dP_d1 = A.get<float>(hwp * nd);
-    v.dRaw_d1 = A.get<float>(hw * nd);
-    const bool in_grad = d.input_grad != 0;   // level 0 then also needs its input gradient
+    const bool d1_dgrad = l > 0 || d.input_grad != 0;   // level 0 has an input gradient with input_grad only
+    if (l == 0) v.Pin = f32("Pin", v.H + 2, v.W + 2, v.Cin, v.Cin);
+    else reg(pf + "Pin", v.Pin = P->lv[l - 1].P_d2, v.H + 2, v.W + 2, v.Cin, v.Cin);
+    v.raw_s = f32("raw_s", v.H, v.W, CS, CS);
+    v.raw_d1 = f32("raw_d1", v.h, v.w, nd, nd);
+    v.P_d1 = f32("P_d1", v.h + 2, v.w + 2, nd, nd);
+    v.raw_d2 = f32("raw_d2", v.h, v.w, nd, nd);
+    v.P_d2 = last ? f32("P_d2", v.h, v.w, nd, nd) : f32("P_d2", v.h + 2, v.w + 2, nd, nd);
+    v.P_cat = f32("P_cat", v.H + 2, v.W + 2, CC, CC);
+    v.raw_u = f32("raw_u", v.H, v.W, nu, nu);
+    v.A_u = f32("A_u", v.H, v.W, nu, nu);
+    v.raw_v = f32("raw_v", v.H, v.W, nu, nu);
+    v.U = (l > 0 || nu != 128) ? f32("U", v.H, v.W, nu, nu) : nullptr;  // a 128-deep level 0 feeds the fused RGB head instead
+    v.dRaw_v = f32("dRaw_v", v.H, v.W, nu, nu);
+    v.dA_u = f32("dA_u", v.H, v.W, nu, nu);
+    v.dRaw_u = f32("dRaw_u", v.H, v.W, nu, nu);
+    v.dP_cat = f32("dP_cat", v.H + 2, v.W + 2, CC, CC);
+    v.dCat = f32("dCat", v.H, v.W, CC, CC);
+    v.dRaw_s = f32("dRaw_s", v.H, v.W, CS, CS);
+    v.dUp = f32("dUp", v.h, v.w, v.cu, v.cu);
+    v.dRaw_d2 = f32("dRaw_d2", v.h, v.w, nd, nd);
+    v.dP_d1 = f32("dP_d1", v.h + 2, v.w + 2, nd, nd);
+    v.dRaw_d1 = f32("dRaw_d1", v.h, v.w, nd, nd);
     if (avg) {
-      v.rawF = A.get<float>(HW * nd);
-      v.dRawF = A.get<float>(HW * nd);
-      if (bf) v.dRawF16 = A.get<uint16_t>(HW * nd);
+      v.rawF = f32("rawF", v.H, v.W, nd, nd);
+      if (bf) v.dRawF16 = b16("dRawF16", v.H, v.W, nd, nd);   // bf16 mode writes the conv's dY as the twin only
+      else v.dRawF = f32("dRawF", v.H, v.W, nd, nd);
     }
-    v.ZS = (l > 0 || in_grad) ? A.get<float>(HW * nd) : nullptr;
-    v.dS = ((wide && l > 0) || (in_grad && l == 0)) ? A.get<float>(HW * v.Cin) : nullptr;
-    v.dPin = (l > 0 || in_grad) ? A.get<float>(HWp * v.Cin) : nullptr;
-    if (bf) {
-      v.Pin_ld16 = round_up(v.Cin, 8); v.cat_ld16 = round_up(CC, 8);
-      if (l == 0) v.Pin16 = A.get<uint16_t>(HWp * v.Pin_ld16); else v.Pin16 = P->lv[l - 1].P_d2_16;
-      v.P_d1_16 = A.get<uint16_t>(hwp * nd);
-      v.P_d2_16 = last ? nullptr : A.get<uint16_t>(hwp * nd);
-      v.P_cat16 = A.get<uint16_t>(HWp * v.cat_ld16);
-      v.A_u16 = A.get<uint16_t>(HW * nu);
-      v.dRaw_v16 = A.get<uint16_t>(HW * nu);
-      v.dRaw_u16 = A.get<uint16_t>(HW * nu);
-      v.dRaw_d2_16 = A.get<uint16_t>(hw * nd);
-      v.dRaw_d1_16 = A.get<uint16_t>(hw * nd);
-      v.dRaw_s16 = wide ? A.get<uint16_t>(HW * 128) : nullptr;
-    }
-    reg(pf + "Pin", v.Pin, v.H + 2, v.W + 2, v.Cin, v.Cin);
-    reg(pf + "raw_s", v.raw_s, v.H, v.W, CS, CS);
-    reg(pf + "raw_d1", v.raw_d1, v.h, v.w, nd, nd);
-    reg(pf + "P_d1", v.P_d1, v.h + 2, v.w + 2, nd, nd);
-    reg(pf + "raw_d2", v.raw_d2, v.h, v.w, nd, nd);
-    if (last) reg(pf + "P_d2", v.P_d2, v.h, v.w, nd, nd); else reg(pf + "P_d2", v.P_d2, v.h + 2, v.w + 2, nd, nd);
-    reg(pf + "P_cat", v.P_cat, v.H + 2, v.W + 2, CC, CC);
-    reg(pf + "raw_u", v.raw_u, v.H, v.W, nu, nu);
-    reg(pf + "A_u", v.A_u, v.H, v.W, nu, nu);
-    reg(pf + "raw_v", v.raw_v, v.H, v.W, nu, nu);
-    if (v.U != nullptr) reg(pf + "U", v.U, v.H, v.W, nu, nu);
-    reg(pf + "dRaw_v", v.dRaw_v, v.H, v.W, nu, nu);
-    reg(pf + "dA_u", v.dA_u, v.H, v.W, nu, nu);
-    reg(pf + "dRaw_u", v.dRaw_u, v.H, v.W, nu, nu);
-    reg(pf + "dP_cat", v.dP_cat, v.H + 2, v.W + 2, CC, CC);
-    reg(pf + "dCat", v.dCat, v.H, v.W, CC, CC);
-    reg(pf + "dRaw_s", v.dRaw_s, v.H, v.W, CS, CS);
-    reg(pf + "dRaw_d2", v.dRaw_d2, v.h, v.w, nd, nd);
-    reg(pf + "dP_d1", v.dP_d1, v.h + 2, v.w + 2, nd, nd);
-    reg(pf + "dRaw_d1", v.dRaw_d1, v.h, v.w, nd, nd);
-    if (bf) {   // bf16 twins of the conv operands (names end in "16": the host side views them as bf16)
-      reg(pf + "Pin16", v.Pin16, v.H + 2, v.W + 2, v.Pin_ld16, v.Cin);
-      reg(pf + "P_d1_16", v.P_d1_16, v.h + 2, v.w + 2, nd, nd);
-      if (!last) reg(pf + "P_d2_16", v.P_d2_16, v.h + 2, v.w + 2, nd, nd);
-      reg(pf + "P_cat16", v.P_cat16, v.H + 2, v.W + 2, v.cat_ld16, CC);
-      reg(pf + "A_u16", v.A_u16, v.H, v.W, nu, nu);
-      reg(pf + "dRaw_v16", v.dRaw_v16, v.H, v.W, nu, nu);
-      reg(pf + "dRaw_u16", v.dRaw_u16, v.H, v.W, nu, nu);
-      reg(pf + "dRaw_d2_16", v.dRaw_d2_16, v.h, v.w, nd, nd);
-      if (!avg) reg(pf + "dRaw_d1_16", v.dRaw_d1_16, v.h, v.w, nd, nd);   // (avg: the pooled gradient stays fp32)
-      if (wide) reg(pf + "dRaw_s16", v.dRaw_s16, v.H, v.W, 128, 128);
-    }
-    reg(pf + "dUp", v.dUp, v.h, v.w, v.cu, v.cu);
-    if (avg) {
-      reg(pf + "rawF", v.rawF, v.H, v.W, nd, nd);
-      if (bf) reg(pf + "dRawF16", v.dRawF16, v.H, v.W, nd, nd);   // bf16 mode writes the conv's dY as the twin only
-      else reg(pf + "dRawF", v.dRawF, v.H, v.W, nd, nd);
-    }
-    if (v.dS != nullptr && CS > 0) reg(pf + "dS", v.dS, v.H, v.W, v.Cin, v.Cin);   // (written by the skip conv's dgrad only)
-    if (v.ZS != nullptr) reg(pf + "ZS", v.ZS, v.H, v.W, nd, nd);
+    // the exact-fp32 mode's stride-2 input gradient reads its dY zero-stuffed
+    v.ZS = (!is_tc(prec) && !avg && d1_dgrad) ? f32("ZS", v.H, v.W, nd, nd) : nullptr;
+    // input gradient of the skip conv: the tensor-core 1x1 of skip=128 (levels > 0), or at level 0 the skip conv's part
+    // of the network's input gradient
+    v.dS = (CS > 0 && (l > 0 ? wide : d.input_grad != 0)) ? f32("dS", v.H, v.W, v.Cin, v.Cin) : nullptr;
     // (level 0: the input gradient conv writes the real input depth only; the stored depth's extra channels are never
     // written, and k_input_grad never reads them)
-    if (v.dPin != nullptr) reg(pf + "dPin", v.dPin, v.H + 2, v.W + 2, v.Cin, v.Cin_act);
+    v.dPin = d1_dgrad ? f32("dPin", v.H + 2, v.W + 2, v.Cin, v.Cin_act) : nullptr;
+    if (bf) {   // bf16 twins of the conv operands (ld = the fp32 tensor's depth rounded up to 8)
+      v.Pin_ld16 = round_up(v.Cin, 8); v.cat_ld16 = round_up(CC, 8);
+      if (l == 0) v.Pin16 = b16("Pin16", v.H + 2, v.W + 2, v.Pin_ld16, v.Cin);
+      else reg(pf + "Pin16", v.Pin16 = P->lv[l - 1].P_d2_16, v.H + 2, v.W + 2, v.Pin_ld16, v.Cin);
+      v.P_d1_16 = b16("P_d1_16", v.h + 2, v.w + 2, nd, nd);
+      v.P_d2_16 = last ? nullptr : b16("P_d2_16", v.h + 2, v.w + 2, nd, nd);
+      v.P_cat16 = b16("P_cat16", v.H + 2, v.W + 2, v.cat_ld16, CC);
+      v.A_u16 = b16("A_u16", v.H, v.W, nu, nu);
+      v.dRaw_v16 = b16("dRaw_v16", v.H, v.W, nu, nu);
+      v.dRaw_u16 = b16("dRaw_u16", v.H, v.W, nu, nu);
+      v.dRaw_d2_16 = b16("dRaw_d2_16", v.h, v.w, nd, nd);
+      v.dRaw_d1_16 = avg ? nullptr : b16("dRaw_d1_16", v.h, v.w, nd, nd);   // (avg: the pooled gradient stays fp32)
+      v.dRaw_s16 = wide ? b16("dRaw_s16", v.H, v.W, 128, 128) : nullptr;
+    }
   }
   P->out_saved = A.get<float>((size_t)P->H * P->W * d.out_channels);
   P->zbuf = A.get<float>((size_t)P->H * P->W * d.in_channels);
@@ -968,16 +950,16 @@ static int build_plan(dip_plan* P, Arena& A) {
       op->wp_f = op->do_fprop ? A.get<float>(op->wp_f_elems()) : nullptr;
       op->wp_d = op->has_dgrad ? A.get<float>(op->wp_d_elems()) : nullptr;
       op->bf16 = bf;
-      op->timer = &P->timer;
+      op->rec = &P->rec;
       const size_t pe = op->do_wgrad ? op->partial_elems(prec) : 0;
       if (pe > partial_max) partial_max = pe;
       P->convs.push_back(op);
     }
   }
   // split-K partials of the weight gradients.  fp32 mode: one area that every conv's wgrad writes and its own unpack entry
-  // sums right away (the tensor-core modes reserve it as well but do not use it).  Tensor-core modes: every conv's partials
-  // in their own slice of one contiguous area, summed by one launch over all entries at the end of the backward pass.
-  P->partial = A.get<float>(partial_max);
+  // sums right away.  Tensor-core modes: every conv's partials in their own slice of one contiguous area, summed by one
+  // launch over all entries at the end of the backward pass.
+  P->partial = is_tc(prec) ? nullptr : A.get<float>(partial_max);
   P->n_unpack = 0;
   for (ConvOp* op : P->convs) if (op->do_wgrad) P->n_unpack++;
   if (is_tc(prec)) {
@@ -1114,7 +1096,7 @@ static const float* level_usrc(const dip_plan* P, int l) {
   return l == L - 1 ? P->lv[l].P_d2 : P->lv[l + 1].U;
 }
 
-static int fwd_level(dip_plan* P, int l, cudaStream_t s, int& nl) {
+static int fwd_level(dip_plan* P, int l, cudaStream_t s) {
   Level& v = P->lv[l];
   const int prec = P->desc.precision;
   const int CS = v.ns, nd = v.nd, nu = v.nu;
@@ -1125,62 +1107,55 @@ static int fwd_level(dip_plan* P, int l, cudaStream_t s, int& nl) {
   // skip branch: 1x1 conv Cin -> CS (+ statistics); independent of the deeper branch until the concat -> skip stream
   if (CS > 0) {
     cudaStream_t ks = fork_skip(P, s);
-    if (CS == 128) {
+    if (CS == 128)
       DIP_CHECK(v.sk.run_fprop(prec, P->params[v.p_skip_b], ks));
-      nl += prec == DIP_PRECISION_FP32 ? 2 : 1;
-    } else {
-      HBM_T(&P->timer, H_SKINNY_FWD, 0, (double)v.H * v.W * (v.Cin_act + CS) * sizeof(float), ks,
-            launch_skinny_fwd(pin_interior, v.Cin, v.W + 2, P->params[v.p_skip_w], P->params[v.p_skip_b], v.Cin, CS, v.H, v.W, v.raw_s, 0,
-                              v.bn_s.fwd, ks, v.Cin_act));
-      nl += 1;
-    }
+    else
+      ENQ(&P->rec, hbm(H_SKINNY_FWD, 0), (double)v.H * v.W * (v.Cin_act + CS) * sizeof(float), ks,
+          launch_skinny_fwd(pin_interior, v.Cin, v.W + 2, P->params[v.p_skip_w], P->params[v.p_skip_b], v.Cin, CS, v.H, v.W, v.raw_s, 0,
+                            v.bn_s.fwd, ks, v.Cin_act));
   }
   // deeper branch
   DIP_CHECK(v.d1.run_fprop(prec, P->params[v.d1.p_b], s));
   if (v.rawF != nullptr) {   // downsample_mode 'avg': pool the stride-1 conv output, then the statistics of the pooled tensor
-    launch_avgpool2(v.rawF, v.h, v.w, nd, v.raw_d1, s);
-    launch_channel_stats(v.raw_d1, nd, nd, v.h * v.w, v.bn_d1.fwd, s);
-    nl += 2;
+    ENQ(&P->rec, kUntimed, 0, s, launch_avgpool2(v.rawF, v.h, v.w, nd, v.raw_d1, s));
+    ENQ(&P->rec, kUntimed, 0, s, launch_channel_stats(v.raw_d1, nd, nd, v.h * v.w, v.bn_d1.fwd, s));
   }
-  HBM_T(&P->timer, H_BN_ACT_WRITE, 1, (double)nd * ((double)v.h * v.w + (double)(v.h + 2) * (v.w + 2)) * sizeof(float), s,
-        launch_bn_act_write(v.raw_d1, nd, bn_ref(P, v.bn_d1), v.h, v.w, bf ? nullptr : v.P_d1, nd, 1, 1, P->act_fun, s, Twin{v.P_d1_16, nd},
-                            P->zero_pad));
+  ENQ(&P->rec, hbm(H_BN_ACT_WRITE, 1), (double)nd * ((double)v.h * v.w + (double)(v.h + 2) * (v.w + 2)) * sizeof(float), s,
+      launch_bn_act_write(v.raw_d1, nd, bn_ref(P, v.bn_d1), v.h, v.w, bf ? nullptr : v.P_d1, nd, 1, 1, P->act_fun, s, Twin{v.P_d1_16, nd},
+                          P->zero_pad));
   DIP_CHECK(v.d2.run_fprop(prec, P->params[v.d2.p_b], s));
-  HBM_T(&P->timer, H_BN_ACT_WRITE, last ? 0 : 1,
-        (double)nd * ((double)v.h * v.w + (last ? (double)v.h * v.w : (double)(v.h + 2) * (v.w + 2))) * sizeof(float), s,
-        launch_bn_act_write(v.raw_d2, nd, bn_ref(P, v.bn_d2), v.h, v.w, (bf && !last && P->lv[l + 1].ns != 4) ? nullptr : v.P_d2, nd, last ? 0 : 1, 1, P->act_fun, s,
-                            Twin{last ? nullptr : v.P_d2_16, nd}, P->zero_pad));   // (the 4-channel skip conv of the next level reads the fp32 tensor)
-  nl += 4 + (prec == DIP_PRECISION_FP32 ? 2 : 0);
-  if (!last) DIP_CHECK(fwd_level(P, l + 1, s, nl));
+  ENQ(&P->rec, hbm(H_BN_ACT_WRITE, last ? 0 : 1),
+      (double)nd * ((double)v.h * v.w + (last ? (double)v.h * v.w : (double)(v.h + 2) * (v.w + 2))) * sizeof(float), s,
+      launch_bn_act_write(v.raw_d2, nd, bn_ref(P, v.bn_d2), v.h, v.w, (bf && !last && P->lv[l + 1].ns != 4) ? nullptr : v.P_d2, nd, last ? 0 : 1, 1, P->act_fun, s,
+                          Twin{last ? nullptr : v.P_d2_16, nd}, P->zero_pad));   // (the 4-channel skip conv of the next level reads the fp32 tensor)
+  if (!last) DIP_CHECK(fwd_level(P, l + 1, s));
   // upsample + concat + BN + pad
   if (CS > 0) join_skip(P, s);
   CatArgs ca = cat_args(P, v, level_usrc(P, l));
   const double cat_in = ((double)v.cu * v.h * v.w + (double)CS * v.H * v.W) * sizeof(float);
-  HBM_T(&P->timer, H_CAT_STATS, v.bilinear, cat_in, s, launch_cat_stats(ca, v.bn_cat.fwd, P->act_fun, s));
-  HBM_T(&P->timer, H_CAT_WRITE, v.bilinear, cat_in + ((double)v.cu + CS) * (v.H + 2) * (v.W + 2) * sizeof(float), s,
-        launch_cat_write(ca, bn_ref(P, v.bn_cat), v.P_cat, P->act_fun, s, Twin{v.P_cat16, v.cat_ld16}, P->zero_pad));
+  ENQ(&P->rec, hbm(H_CAT_STATS, v.bilinear), cat_in, s, launch_cat_stats(ca, v.bn_cat.fwd, P->act_fun, s));
+  ENQ(&P->rec, hbm(H_CAT_WRITE, v.bilinear), cat_in + ((double)v.cu + CS) * (v.H + 2) * (v.W + 2) * sizeof(float), s,
+      launch_cat_write(ca, bn_ref(P, v.bn_cat), v.P_cat, P->act_fun, s, Twin{v.P_cat16, v.cat_ld16}, P->zero_pad));
   DIP_CHECK(v.up.run_fprop(prec, P->params[v.up.p_b], s));
-  HBM_T(&P->timer, H_BN_ACT_WRITE, 0, 2.0 * nu * v.H * v.W * sizeof(float), s,
-        launch_bn_act_write(v.raw_u, nu, bn_ref(P, v.bn_u), v.H, v.W, bf ? nullptr : v.A_u, nu, 0, 1, P->act_fun, s, Twin{v.A_u16, nu}));
+  ENQ(&P->rec, hbm(H_BN_ACT_WRITE, 0), 2.0 * nu * v.H * v.W * sizeof(float), s,
+      launch_bn_act_write(v.raw_u, nu, bn_ref(P, v.bn_u), v.H, v.W, bf ? nullptr : v.A_u, nu, 0, 1, P->act_fun, s, Twin{v.A_u16, nu}));
   DIP_CHECK(v.c11.run_fprop(prec, P->params[v.c11.p_b], s));
   if (l > 0 || nu != 128) {
-    HBM_T(&P->timer, H_BN_ACT_WRITE, 0, 2.0 * nu * v.H * v.W * sizeof(float), s,
-          launch_bn_act_write(v.raw_v, nu, bn_ref(P, v.bn_v), v.H, v.W, v.U, nu, 0, 1, P->act_fun, s));
+    ENQ(&P->rec, hbm(H_BN_ACT_WRITE, 0), 2.0 * nu * v.H * v.W * sizeof(float), s,
+        launch_bn_act_write(v.raw_v, nu, bn_ref(P, v.bn_v), v.H, v.W, v.U, nu, 0, 1, P->act_fun, s));
     if (l == 0) {
       // level 0 narrower than 128 channels: the RGB head (models/skip.py:95-98) as a skinny 1x1 conv over the materialised
       // activation (the fused BN + head kernel is specialised for 128 channels = one warp per pixel)
-      HBM_T(&P->timer, H_SKINNY_FWD, 1, ((double)nu + P->desc.out_channels) * v.H * v.W * sizeof(float), s,
-            launch_skinny_fwd(v.U, nu, v.W, P->params[P->p_head_w], P->params[P->p_head_b], nu, P->desc.out_channels, v.H, v.W,
-                              P->out_saved, P->desc.need_sigmoid != 0 ? 1 : 2, nullptr, s));
-      nl += 1;
+      ENQ(&P->rec, hbm(H_SKINNY_FWD, 1), ((double)nu + P->desc.out_channels) * v.H * v.W * sizeof(float), s,
+          launch_skinny_fwd(v.U, nu, v.W, P->params[P->p_head_w], P->params[P->p_head_b], nu, P->desc.out_channels, v.H, v.W,
+                            P->out_saved, P->desc.need_sigmoid != 0 ? 1 : 2, nullptr, s));
     }
   } else {
     // top level: BN + activation + RGB head + sigmoid in one pass; the 128-channel activation is never materialised
     HeadRef hd{P->params[P->p_head_w], P->params[P->p_head_b], P->desc.out_channels, P->out_saved, P->desc.need_sigmoid != 0};
-    HBM_T(&P->timer, H_BN_ACT_HEAD, 0, (128.0 + P->desc.out_channels) * v.H * v.W * sizeof(float), s,
-          launch_bn_act_head(v.raw_v, bn_ref(P, v.bn_v), v.H, v.W, hd, P->act_fun, s));
+    ENQ(&P->rec, hbm(H_BN_ACT_HEAD, 0), (128.0 + P->desc.out_channels) * v.H * v.W * sizeof(float), s,
+        launch_bn_act_head(v.raw_v, bn_ref(P, v.bn_v), v.H, v.W, hd, P->act_fun, s));
   }
-  nl += 6 + (prec == DIP_PRECISION_FP32 ? 2 : 0);
   DIP_CUDA(cudaGetLastError());
   return 0;
 }
@@ -1191,42 +1166,40 @@ static void plan_pack(dip_plan* P, cudaStream_t s) {
   double bytes = 0;
   for (ConvOp* op : P->convs)
     bytes += ((double)op->N * op->C * op->k * op->k + (op->do_fprop ? (double)op->wp_f_elems() : 0.0) + (op->has_dgrad ? (double)op->wp_d_elems() : 0.0)) * sizeof(float);
-  HBM_T(&P->timer, H_PACK, 0, bytes, s, launch_k(k_pack_table, dim3(grid), dim3(256), 0, s, 1, P->d_pack));
+  ENQ(&P->rec, hbm(H_PACK, 0), bytes, s, launch_k(k_pack_table, dim3(grid), dim3(256), 0, s, 1, P->d_pack));
 }
 
 static int plan_forward(dip_plan* P, const float* z, const float* noise, float sigma, float* out, cudaStream_t s) {
   if (!P->bound) return fail("dip_forward: parameters not bound (call dip_plan_bind)");
   // grid-wide reductions: fp64 atomics onto line-strided accumulators (default) or the deterministic last-block sum
-  int nl = 0;
   P->side_on = getenv("DIP_NO_SIDE") == nullptr;
-  if (!P->prepacked) P->wev_used = 0;
-  DIP_CUDA(cudaMemsetAsync(P->acc_fwd, 0, P->acc_fwd_n * sizeof(double), s));
+  if (!P->prepacked) { P->wev_used = 0; P->rec.n = 0; }
+  ENQ(&P->rec, kUntimed, 0, s, DIP_CUDA(cudaMemsetAsync(P->acc_fwd, 0, P->acc_fwd_n * sizeof(double), s)));
   if (!P->prepacked) plan_pack(P, fork_side(P, s));   // weight repack runs beside the input transform
   P->prepacked = false;
   Level& v0 = P->lv[0];
   if (P->fnoise.on)
-    HBM_T(&P->timer, H_NOISE, 1, ((double)v0.Cin_act * v0.H * v0.W + (double)v0.Cin * (v0.H + 2) * (v0.W + 2)) * sizeof(float), s,
-          launch_noise_pad(P->fnoise.z0, P->fnoise.sigma, P->fnoise.seed, P->fnoise.offset, P->fnoise.it_dev, v0.Pin, v0.Cin,
-                           v0.H, v0.W, v0.Cin_act, s, Twin{v0.Pin16, v0.Pin_ld16}, P->zero_pad));
+    ENQ(&P->rec, hbm(H_NOISE, 1), ((double)v0.Cin_act * v0.H * v0.W + (double)v0.Cin * (v0.H + 2) * (v0.W + 2)) * sizeof(float), s,
+        launch_noise_pad(P->fnoise.z0, P->fnoise.sigma, P->fnoise.seed, P->fnoise.offset, P->fnoise.it_dev, v0.Pin, v0.Cin,
+                         v0.H, v0.W, v0.Cin_act, s, Twin{v0.Pin16, v0.Pin_ld16}, P->zero_pad));
   else
-    HBM_T(&P->timer, H_INPUT_PAD, noise != nullptr,
-          ((noise != nullptr ? 2.0 : 1.0) * v0.Cin_act * v0.H * v0.W + (double)v0.Cin * (v0.H + 2) * (v0.W + 2)) * sizeof(float), s,
-          launch_input_pad(z, noise, sigma, v0.Pin, v0.Cin, v0.H, v0.W, s, v0.Cin_act, Twin{v0.Pin16, v0.Pin_ld16}, P->zero_pad));
+    ENQ(&P->rec, hbm(H_INPUT_PAD, noise != nullptr),
+        ((noise != nullptr ? 2.0 : 1.0) * v0.Cin_act * v0.H * v0.W + (double)v0.Cin * (v0.H + 2) * (v0.W + 2)) * sizeof(float), s,
+        launch_input_pad(z, noise, sigma, v0.Pin, v0.Cin, v0.H, v0.W, s, v0.Cin_act, Twin{v0.Pin16, v0.Pin_ld16}, P->zero_pad));
   join_side(P, s);
-  nl += 3;
-  DIP_CHECK(fwd_level(P, 0, s, nl));
+  DIP_CHECK(fwd_level(P, 0, s));
   if (out != nullptr && out != P->out_saved)
-    DIP_CUDA(cudaMemcpyAsync(out, P->out_saved, (size_t)v0.H * v0.W * P->desc.out_channels * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  launch_k(k_running_table, dim3(P->n_run), dim3(160), 0, s, 1, P->d_run);
-  nl += 3;
+    ENQ(&P->rec, kUntimed, 0, s,
+        DIP_CUDA(cudaMemcpyAsync(out, P->out_saved, (size_t)v0.H * v0.W * P->desc.out_channels * sizeof(float), cudaMemcpyDeviceToDevice, s)));
+  ENQ(&P->rec, kUntimed, 0, s, launch_k(k_running_table, dim3(P->n_run), dim3(160), 0, s, 1, P->d_run));
   DIP_CUDA(cudaGetLastError());
-  P->launches_fwd = nl;
+  P->launches_fwd = P->rec.n;
   return 0;
 }
 
 // ------------------------------------------------------------------------------------------------ backward
 static int bn_bwd(dip_plan* P, const float* raw, int ld_raw, BnLayer& b, int act, GradSrc src, int H, int W, float* draw,
-                  float* zs, cudaStream_t s, int& nl, uint16_t* draw16 = nullptr) {
+                  float* zs, cudaStream_t s, uint16_t* draw16 = nullptr) {
   if (draw16 != nullptr && zs == nullptr) draw = nullptr;   // bf16 mode: only the tensor-core dgrad / wgrad read this gradient
   if (src.kind == 1) src.zero_pad = P->zero_pad;            // zero padding: the padded gradient's halo is dropped, not folded
   BnRef r = bn_ref(P, b);
@@ -1238,10 +1211,9 @@ static int bn_bwd(dip_plan* P, const float* raw, int ld_raw, BnLayer& b, int act
   if (src.kind == 1) gsrc = (src.zero_pad ? px : (double)(H + 2) * (W + 2)) * C4 + (src.ds != nullptr ? px * 4 * sizeof(float) : 0.0) + (src.add != nullptr ? px * C4 : 0.0);
   else if (src.kind == 2) gsrc = 4.0 * px * C4;
   else if (src.kind == 3) gsrc = px * 4 * sizeof(float);
-  HBM_T(&P->timer, H_BN_BWD_REDUCE, src.kind, px * C4 + gsrc, s, launch_bn_bwd_reduce(raw, ld_raw, r, act, P->act_fun, src, H, W, b.bwd, s));
-  HBM_T(&P->timer, H_BN_BWD_APPLY, src.kind + (zs != nullptr ? 4 : 0), px * C4 + gsrc + px * C4 * (zs != nullptr ? 2.0 : 1.0), s,
-        launch_bn_bwd_apply(raw, ld_raw, r, act, P->act_fun, src, H, W, b.bwd, draw, zs, b.dbias, s, Twin{draw16, b.C}));
-  nl += 2;
+  ENQ(&P->rec, hbm(H_BN_BWD_REDUCE, src.kind), px * C4 + gsrc, s, launch_bn_bwd_reduce(raw, ld_raw, r, act, P->act_fun, src, H, W, b.bwd, s));
+  ENQ(&P->rec, hbm(H_BN_BWD_APPLY, src.kind + (zs != nullptr ? 4 : 0)), px * C4 + gsrc + px * C4 * (zs != nullptr ? 2.0 : 1.0), s,
+      launch_bn_bwd_apply(raw, ld_raw, r, act, P->act_fun, src, H, W, b.bwd, draw, zs, b.dbias, s, Twin{draw16, b.C}));
   return 0;
 }
 static GradSrc src_plain(const float* g, int ld, int coff) { GradSrc s{}; s.kind = 0; s.g = g; s.ld = ld; s.coff = coff; return s; }
@@ -1276,63 +1248,56 @@ static int conv_backward(dip_plan* P, ConvOp& op, bool dgrad, int prec, cudaStre
   return op.run_wgrad(prec, ws);
 }
 
-static int bwd_level(dip_plan* P, int l, GradSrc src_v, cudaStream_t s, int& nl) {
+static int bwd_level(dip_plan* P, int l, GradSrc src_v, cudaStream_t s) {
   Level& v = P->lv[l];
   const int prec = P->desc.precision;
   const int CS = v.ns, nd = v.nd, nu = v.nu;
   const int CC = v.cu + CS;
   const bool last = l == (int)P->lv.size() - 1;
-  const int wl = is_tc(prec) ? 1 : 2;   // fp32 mode: every wgrad is followed by its own split-K sum
   // 1x1 conv + BN + LReLU
-  DIP_CHECK(bn_bwd(P, v.raw_v, nu, v.bn_v, 1, src_v, v.H, v.W, v.dRaw_v, nullptr, s, nl, v.dRaw_v16));
+  DIP_CHECK(bn_bwd(P, v.raw_v, nu, v.bn_v, 1, src_v, v.H, v.W, v.dRaw_v, nullptr, s, v.dRaw_v16));
   if (l == kDeferLevel) DIP_CHECK(flush_deferred(P, prec, s));
   DIP_CHECK(conv_backward(P, v.c11, true, prec, s, l));
-  nl += wl + 1;
   // up conv + BN + LReLU
-  DIP_CHECK(bn_bwd(P, v.raw_u, nu, v.bn_u, 1, src_plain(v.dA_u, nu, 0), v.H, v.W, v.dRaw_u, nullptr, s, nl, v.dRaw_u16));
+  DIP_CHECK(bn_bwd(P, v.raw_u, nu, v.bn_u, 1, src_plain(v.dA_u, nu, 0), v.H, v.W, v.dRaw_u, nullptr, s, v.dRaw_u16));
   if (CS == 128) {
     cudaStream_t ws = fork_side(P, s);
     DIP_CHECK(v.up_a.run_dgrad(prec, s));
     DIP_CHECK(v.up_b.run_dgrad(prec, s));
     DIP_CHECK(v.up_a.run_wgrad(prec, ws));
     DIP_CHECK(v.up_b.run_wgrad(prec, ws));
-    nl += 2 * (wl + 1);
   } else {
     DIP_CHECK(conv_backward(P, v.up, true, prec, s, l));
-    nl += wl + 1;
   }
   // concat BN
   BnRef rc = bn_ref(P, v.bn_cat);
   // stored BN output + padded gradient (zero padding: its interior only)
   const double catb = ((double)v.H * v.W + (P->zero_pad ? (double)v.H * v.W : (double)(v.H + 2) * (v.W + 2))) * CC * sizeof(float);
-  HBM_T(&P->timer, H_CAT_BWD_REDUCE, 0, catb, s, launch_cat_bwd_reduce(v.P_cat, rc, v.dP_cat, CC, v.H, v.W, v.bn_cat.bwd, s, P->zero_pad));
-  HBM_T(&P->timer, H_CAT_BWD_APPLY, 0, catb + (double)v.H * v.W * CC * sizeof(float), s,
-        launch_cat_bwd_apply(v.P_cat, rc, v.dP_cat, CC, v.H, v.W, v.bn_cat.bwd, v.dCat, s, P->zero_pad));
+  ENQ(&P->rec, hbm(H_CAT_BWD_REDUCE, 0), catb, s, launch_cat_bwd_reduce(v.P_cat, rc, v.dP_cat, CC, v.H, v.W, v.bn_cat.bwd, s, P->zero_pad));
+  ENQ(&P->rec, hbm(H_CAT_BWD_APPLY, 0), catb + (double)v.H * v.W * CC * sizeof(float), s,
+      launch_cat_bwd_apply(v.P_cat, rc, v.dP_cat, CC, v.H, v.W, v.bn_cat.bwd, v.dCat, s, P->zero_pad));
   // skip branch (on the skip stream: independent of the deeper levels; the level above joins before it reads dRaw_s / dS)
   cudaStream_t ks = fork_skip(P, s);
   // gradient w.r.t. the low-resolution tensor that was upsampled into this concat (adjoint of x2 upsampling), once
-  HBM_T(&P->timer, H_UPADJ, v.bilinear, (double)v.cu * ((double)v.H * v.W + (double)v.h * v.w) * sizeof(float), s,
-        launch_upadj(v.dCat, CC, 0, v.h, v.w, v.cu, v.bilinear, v.dUp, s));
-  nl += 3;
-  if (CS > 0) DIP_CHECK(bn_bwd(P, v.raw_s, CS, v.bn_s, 1, src_plain(v.dCat, CC, v.cu), v.H, v.W, v.dRaw_s, nullptr, ks, nl, v.dRaw_s16));
+  ENQ(&P->rec, hbm(H_UPADJ, v.bilinear), (double)v.cu * ((double)v.H * v.W + (double)v.h * v.w) * sizeof(float), s,
+      launch_upadj(v.dCat, CC, 0, v.h, v.w, v.cu, v.bilinear, v.dUp, s));
+  if (CS > 0) DIP_CHECK(bn_bwd(P, v.raw_s, CS, v.bn_s, 1, src_plain(v.dCat, CC, v.cu), v.H, v.W, v.dRaw_s, nullptr, ks, v.dRaw_s16));
   if (CS == 0) {
     // no skip branch (models/skip.py:50-53 with num_channels_skip = 0)
   } else if (CS == 128) {
     DIP_CHECK(v.sk.run_wgrad(prec, fork_side(P, ks)));
-    nl += wl;
-    if (l > 0 || P->desc.input_grad) { DIP_CHECK(v.sk.run_dgrad(prec, ks)); nl += 1; }   // dS, added to the fold of dPin by the level above
+    if (l > 0 || P->desc.input_grad) DIP_CHECK(v.sk.run_dgrad(prec, ks));   // dS, added to the fold of dPin by the level above
   } else {
     const float* pin_interior = v.Pin + ((size_t)(v.W + 2) + 1) * v.Cin;
     // weight gradient only: the input gradient of this conv is folded into the BN backward of the level above
-    HBM_T(&P->timer, H_SKINNY_BWD, 0, (double)v.H * v.W * (v.Cin_act + CS) * sizeof(float), ks,
-          launch_skinny_bwd(pin_interior, v.Cin, v.W + 2, P->params[v.p_skip_w], v.Cin, CS, v.H, v.W, v.dRaw_s, nullptr, 0,
-                            (l == 0 && P->desc.input_grad) ? v.dS : nullptr, v.dw_s, nullptr /*bias grad comes from the BN backward*/, ks, v.Cin_act));
-    nl += 1;
+    ENQ(&P->rec, hbm(H_SKINNY_BWD, 0), (double)v.H * v.W * (v.Cin_act + CS) * sizeof(float), ks,
+        launch_skinny_bwd(pin_interior, v.Cin, v.W + 2, P->params[v.p_skip_w], v.Cin, CS, v.H, v.W, v.dRaw_s, nullptr, 0,
+                          (l == 0 && P->desc.input_grad) ? v.dS : nullptr, v.dw_s, nullptr /*bias grad comes from the BN backward*/, ks, v.Cin_act));
   }
   // deeper branch
   GradSrc src_d2;
   if (!last) {
-    DIP_CHECK(bwd_level(P, l + 1, src_plain(v.dUp, v.cu, 0), s, nl));
+    DIP_CHECK(bwd_level(P, l + 1, src_plain(v.dUp, v.cu, 0), s));
     join_skip(P, s);   // the next level's skip-branch gradients (dRaw_s / dS) feed the BN backward below
     Level& n = P->lv[l + 1];   // (its input depth n.Cin == nd)
     if (n.ns == 128) { src_d2 = src_fold(n.dPin, nd, nullptr, nullptr, 0); src_d2.add = n.dS; src_d2.ld_add = nd; }
@@ -1341,50 +1306,43 @@ static int bwd_level(dip_plan* P, int l, GradSrc src_v, cudaStream_t s, int& nl)
   } else {
     src_d2 = src_plain(v.dUp, v.cu, 0);
   }
-  DIP_CHECK(bn_bwd(P, v.raw_d2, nd, v.bn_d2, 1, src_d2, v.h, v.w, v.dRaw_d2, nullptr, s, nl, v.dRaw_d2_16));
+  DIP_CHECK(bn_bwd(P, v.raw_d2, nd, v.bn_d2, 1, src_d2, v.h, v.w, v.dRaw_d2, nullptr, s, v.dRaw_d2_16));
   DIP_CHECK(conv_backward(P, v.d2, true, prec, s));
-  nl += wl + 1;
   const bool d1_dgrad = l > 0 || P->desc.input_grad != 0;
   const bool avg = v.rawF != nullptr;
   DIP_CHECK(bn_bwd(P, v.raw_d1, nd, v.bn_d1, 1, src_fold(v.dP_d1, nd, nullptr, nullptr, 0), v.h, v.w, v.dRaw_d1,
-                   (d1_dgrad && !v.d1.dg_s2 && !avg) ? v.ZS : nullptr, s, nl, avg ? nullptr : v.dRaw_d1_16));
-  if (avg) {   // adjoint of AvgPool2d(2, 2): the conv's dY at full resolution
-    launch_avgpool2_bwd(v.dRaw_d1, v.h, v.w, nd, prec == DIP_PRECISION_BF16 ? nullptr : v.dRawF, s, Twin{v.dRawF16, nd});
-    nl += 1;
-  }
+                   (d1_dgrad && !v.d1.dg_s2 && !avg) ? v.ZS : nullptr, s, avg ? nullptr : v.dRaw_d1_16));
+  if (avg)   // adjoint of AvgPool2d(2, 2): the conv's dY at full resolution
+    ENQ(&P->rec, kUntimed, 0, s,
+        launch_avgpool2_bwd(v.dRaw_d1, v.h, v.w, nd, prec == DIP_PRECISION_BF16 ? nullptr : v.dRawF, s, Twin{v.dRawF16, nd}));
   DIP_CHECK(conv_backward(P, v.d1, d1_dgrad, prec, s));
-  nl += wl + (d1_dgrad ? 1 : 0);
   DIP_CUDA(cudaGetLastError());
   return 0;
 }
 
 static int plan_backward(dip_plan* P, const float* dout, cudaStream_t s) {
   if (!P->bound) return fail("dip_backward: parameters not bound");
-  int nl = 0;
+  P->rec.n = 0;
   P->deferred.clear();
-  DIP_CUDA(cudaMemsetAsync(P->acc_bwd, 0, P->acc_bwd_n * sizeof(double), s));
+  ENQ(&P->rec, kUntimed, 0, s, DIP_CUDA(cudaMemsetAsync(P->acc_bwd, 0, P->acc_bwd_n * sizeof(double), s)));
   P->side_on = getenv("DIP_NO_SIDE") == nullptr;
   Level& v0 = P->lv[0];
   // RGB head backward (sigmoid', dgrad 3->128, wgrad, bias grad) is fused into the BN backward of the last stage
   GradSrc sh{};
-  HBM_T(&P->timer, H_HEAD_DLOGIT, 0, (2.0 * P->desc.out_channels + 4.0) * P->H * P->W * sizeof(float), s,
-        launch_head_dlogit(dout, P->out_saved, P->desc.out_channels, P->H * P->W, P->dl4, s, P->desc.need_sigmoid != 0));
+  ENQ(&P->rec, hbm(H_HEAD_DLOGIT, 0), (2.0 * P->desc.out_channels + 4.0) * P->H * P->W * sizeof(float), s,
+      launch_head_dlogit(dout, P->out_saved, P->desc.out_channels, P->H * P->W, P->dl4, s, P->desc.need_sigmoid != 0));
   sh.kind = 3; sh.dl4 = P->dl4; sh.wh = P->params[P->p_head_w]; sh.nh = P->desc.out_channels;
   sh.dwh = P->dw_head; sh.dbh = P->db_head;
-  nl += 1;
-  DIP_CHECK(bwd_level(P, 0, sh, s, nl));
+  DIP_CHECK(bwd_level(P, 0, sh, s));
   DIP_CHECK(flush_deferred(P, P->desc.precision, s));
   join_side(P, s);
   join_skip(P, s);
-  launch_k(k_cvt_table, dim3(P->n_cvt), dim3(128), 0, s, 1, P->d_cvt);
-  nl += 1;
-  if (is_tc(P->desc.precision) && P->n_unpack > 0) {   // (fp32 mode: each conv's entry ran after its wgrad)
-    HBM_T(&P->timer, H_WGRAD_REDUCE, 1, 2.0 * (double)P->wacc_bytes, s,
-          launch_k(k_wgrad_unpack_table, dim3(64, P->n_unpack), dim3(256), 0, s, 1, P->d_unpack));
-    nl += 1;
-  }
+  ENQ(&P->rec, kUntimed, 0, s, launch_k(k_cvt_table, dim3(P->n_cvt), dim3(128), 0, s, 1, P->d_cvt));
+  if (is_tc(P->desc.precision) && P->n_unpack > 0)   // (fp32 mode: each conv's entry ran after its wgrad)
+    ENQ(&P->rec, hbm(H_WGRAD_REDUCE, 1), 2.0 * (double)P->wacc_bytes, s,
+        launch_k(k_wgrad_unpack_table, dim3(64, P->n_unpack), dim3(256), 0, s, 1, P->d_unpack));
   DIP_CUDA(cudaGetLastError());
-  P->launches_bwd = nl;
+  P->launches_bwd = P->rec.n;
   return 0;
 }
 
@@ -1421,6 +1379,20 @@ static int ensure_gstream(dip_plan* P) {
   }
   return 0;
 }
+// Captures body(gs) into *exec (nullptr on failure).
+template <class Body>
+static int capture_graph(cudaStream_t gs, cudaGraphExec_t* exec, Body body) {
+  cudaGraph_t graph = nullptr;
+  DIP_CUDA(cudaStreamBeginCapture(gs, cudaStreamCaptureModeThreadLocal));
+  const int rc = body(gs);
+  cudaError_t ce = cudaStreamEndCapture(gs, &graph);
+  if (rc != 0) { if (graph) cudaGraphDestroy(graph); return rc; }
+  if (ce != cudaSuccess) return fail(std::string("cudaStreamEndCapture: ") + cudaGetErrorString(ce));
+  ce = cudaGraphInstantiate(exec, graph, 0);
+  cudaGraphDestroy(graph);
+  if (ce != cudaSuccess) { *exec = nullptr; return fail(std::string("cudaGraphInstantiate: ") + cudaGetErrorString(ce)); }
+  return 0;
+}
 // Captures body(gstream) once into *exec, then replays it between two event edges to / from the caller's stream `s`.
 template <class Body>
 static int replay_graph(dip_plan* P, cudaGraphExec_t* exec, cudaStream_t s, Body body) {
@@ -1428,17 +1400,7 @@ static int replay_graph(dip_plan* P, cudaGraphExec_t* exec, cudaStream_t s, Body
   cudaStream_t gs = P->gstream;
   DIP_CUDA(cudaEventRecord(P->gev_in, s));
   DIP_CUDA(cudaStreamWaitEvent(gs, P->gev_in, 0));
-  if (*exec == nullptr) {
-    cudaGraph_t graph = nullptr;
-    DIP_CUDA(cudaStreamBeginCapture(gs, cudaStreamCaptureModeThreadLocal));
-    const int rc = body(gs);
-    cudaError_t ce = cudaStreamEndCapture(gs, &graph);
-    if (rc != 0) { if (graph) cudaGraphDestroy(graph); return rc; }
-    if (ce != cudaSuccess) return fail(std::string("cudaStreamEndCapture: ") + cudaGetErrorString(ce));
-    ce = cudaGraphInstantiate(exec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (ce != cudaSuccess) { *exec = nullptr; return fail(std::string("cudaGraphInstantiate: ") + cudaGetErrorString(ce)); }
-  }
+  if (*exec == nullptr) DIP_CHECK(capture_graph(gs, exec, body));
   DIP_CUDA(cudaGraphLaunch(*exec, gs));
   DIP_CUDA(cudaEventRecord(P->gev_out, gs));
   DIP_CUDA(cudaStreamWaitEvent(s, P->gev_out, 0));
@@ -1651,15 +1613,18 @@ static int run_body(dip_plan* P, dip_adam* adam, const float* z0, const float* t
   const size_t nz = (size_t)P->H * P->W * P->desc.in_channels;
   const int hw = P->H * P->W;
   const float* zin = z0;
+  Recorder runner{&P->timer};   // the runner's own launches: timed like the plan's, not part of its forward / backward counts
   P->side_on = getenv("DIP_NO_SIDE") == nullptr;
   P->wev_used = 0;
   if (P->side_on && P->bound) {
-    // weight repack on the side stream from the very start of the iteration (beside the noise kernel); plan_forward joins it
+    // weight repack on the side stream from the very start of the iteration (beside the noise kernel); plan_forward joins
+    // it, and counts it as its own
+    P->rec.n = 0;
     plan_pack(P, fork_side(P, s));
     P->prepacked = true;
   }
   if (sigma > 0.f && P->W % 4 != 0) {   // the fused k_noise_pad needs W % 4 == 0: separate k_noise + k_input_pad launches
-    HBM_T(&P->timer, H_NOISE, 0, 2.0 * nz * sizeof(float), s, launch_noise(z0, P->zbuf, sigma, seed, (uint64_t)step_base, it_dev, nz, s));
+    ENQ(&runner, hbm(H_NOISE, 0), 2.0 * nz * sizeof(float), s, launch_noise(z0, P->zbuf, sigma, seed, (uint64_t)step_base, it_dev, nz, s));
     zin = P->zbuf;
   } else if (sigma > 0.f) {
     P->fnoise.on = true; P->fnoise.z0 = z0; P->fnoise.sigma = sigma; P->fnoise.seed = seed; P->fnoise.offset = (uint64_t)step_base;
@@ -1673,21 +1638,21 @@ static int run_body(dip_plan* P, dip_adam* adam, const float* z0, const float* t
     // super-resolution: loss on the downsampled output (super-resolution.ipynb c10:8-11); the operator's adjoint
     // turns the low-resolution loss gradient into dL/d(out)
     const int co = P->desc.out_channels;
-    HBM_T(&P->timer, H_DOWN_FWD, 0, (double)co * ((double)P->H * P->W + (double)P->ds_Ho * P->ds_Wo) * sizeof(float), s,
-          DIP_CUDA(launch_down_fwd(P->out_saved, co, P->H, P->W, P->ds_kern, P->ds_K, P->ds_f, P->ds_pad, P->ds_y, s)));
+    ENQ(&runner, hbm(H_DOWN_FWD, 0), (double)co * ((double)P->H * P->W + (double)P->ds_Ho * P->ds_Wo) * sizeof(float), s,
+        DIP_CUDA(launch_down_fwd(P->out_saved, co, P->H, P->W, P->ds_kern, P->ds_K, P->ds_f, P->ds_pad, P->ds_y, s)));
     launch_mse(P->ds_y, target, mask, co, P->ds_Ho * P->ds_Wo, loss_slot, P->ds_dy, slot_idx, s);
-    HBM_T(&P->timer, H_DOWN_BWD, 0, (double)co * ((double)P->H * P->W + (double)P->ds_Ho * P->ds_Wo) * sizeof(float), s,
-          DIP_CUDA(launch_down_bwd(P->ds_dy, co, P->H, P->W, P->ds_kern, P->ds_K, P->ds_f, P->ds_pad, P->dout, s)));
+    ENQ(&runner, hbm(H_DOWN_BWD, 0), (double)co * ((double)P->H * P->W + (double)P->ds_Ho * P->ds_Wo) * sizeof(float), s,
+        DIP_CUDA(launch_down_bwd(P->ds_dy, co, P->H, P->W, P->ds_kern, P->ds_K, P->ds_f, P->ds_pad, P->dout, s)));
   } else {
-    HBM_T(&P->timer, H_MSE, mask != nullptr, (3.0 * P->desc.out_channels + (mask != nullptr ? 1.0 : 0.0)) * hw * sizeof(float), s,
-          launch_mse(P->out_saved, target, mask, P->desc.out_channels, hw, loss_slot, P->dout, slot_idx, s));
+    ENQ(&runner, hbm(H_MSE, mask != nullptr), (3.0 * P->desc.out_channels + (mask != nullptr ? 1.0 : 0.0)) * hw * sizeof(float), s,
+        launch_mse(P->out_saved, target, mask, P->desc.out_channels, hw, loss_slot, P->dout, slot_idx, s));
   }
   DIP_CHECK(plan_backward(P, P->dout, s));
   if (!adam->bound) return fail("dip_run_iterations: adam not bound");
   AdamTable t{adam->d_p, adam->d_g, adam->d_m, adam->d_v, adam->d_blk_tensor, adam->d_blk_start, adam->d_numel, adam->nblocks};
   {
     double np_ = 0; for (long long n : adam->numel) np_ += (double)n;
-    HBM_T(&P->timer, H_ADAM, 0, 7.0 * np_ * sizeof(float), s, launch_adam(t, lr, 0.9, 0.999, 1e-8, step_base + 1, it_dev, s));
+    ENQ(&runner, hbm(H_ADAM, 0), 7.0 * np_ * sizeof(float), s, launch_adam(t, lr, 0.9, 0.999, 1e-8, step_base + 1, it_dev, s));
   }
   if (it_dev != nullptr) launch_advance(it_dev, s);
   DIP_CUDA(cudaGetLastError());
@@ -1727,16 +1692,10 @@ int dip_run_iterations(dip_plan* P, dip_adam* adam, const void* z0, const void* 
   key.adam_id = adam->id; key.adam_bind = adam->bind_gen; key.sigma = sigma; key.seed = seed; key.lr = lr;
   if (P->gexec == nullptr || !(key == P->gkey)) {
     if (P->gexec != nullptr) { cudaGraphExecDestroy(P->gexec); P->gexec = nullptr; }
-    cudaGraph_t graph = nullptr;
-    DIP_CUDA(cudaStreamBeginCapture(gs, cudaStreamCaptureModeThreadLocal));
-    const int rc = run_body(P, adam, (const float*)z0, (const float*)target, (const float*)mask, sigma, seed, 0, lr, (float*)out,
-                            slots, P->it_dev, gs);
-    cudaError_t ce = cudaStreamEndCapture(gs, &graph);
-    if (rc != 0) { if (graph) cudaGraphDestroy(graph); return rc; }
-    if (ce != cudaSuccess) return fail(std::string("cudaStreamEndCapture: ") + cudaGetErrorString(ce));
-    ce = cudaGraphInstantiate(&P->gexec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (ce != cudaSuccess) { P->gexec = nullptr; return fail(std::string("cudaGraphInstantiate: ") + cudaGetErrorString(ce)); }
+    DIP_CHECK(capture_graph(gs, &P->gexec, [&](cudaStream_t cs) {
+      return run_body(P, adam, (const float*)z0, (const float*)target, (const float*)mask, sigma, seed, 0, lr, (float*)out, slots,
+                      P->it_dev, cs);
+    }));
     P->gkey = key;
   }
   const int init[2] = {step0, 0};
