@@ -163,7 +163,7 @@ struct Recorder {
 // reads + writes, x 4 B; SURVEY.md 8d) -- bench.py's HBM rooflines.  kUntimed: counted only.
 enum HbmId { H_INPUT_PAD = 0, H_NOISE, H_SKINNY_FWD, H_BN_ACT_WRITE, H_BN_ACT_HEAD, H_CAT_STATS, H_CAT_WRITE, H_BN_BWD_REDUCE,
              H_BN_BWD_APPLY, H_CAT_BWD_REDUCE, H_CAT_BWD_APPLY, H_UPADJ, H_SKINNY_BWD, H_MSE, H_ADAM, H_HEAD_DLOGIT, H_DOWN_FWD,
-             H_DOWN_BWD, H_PACK, H_WGRAD_REDUCE };
+             H_DOWN_BWD, H_PACK, H_WGRAD_REDUCE, H_TRACK_OUT, H_TRACK_DECIDE, H_ADAM_TRACK };
 static constexpr int kUntimed = -1;
 static int hbm(HbmId id, int sub) { return 16 + 8 * (int)id + sub; }
 struct EnqScope {
@@ -613,9 +613,13 @@ struct dip_plan {
     const void *z0 = nullptr, *target = nullptr, *mask = nullptr, *out = nullptr, *slots = nullptr;
     unsigned long long adam_id = 0, adam_bind = 0;
     float sigma = 0.f; uint64_t seed = 0; double lr = 0.0;
+    dip_track track{};   // all zero when the runner is untracked (a tracker always has out_avg != NULL)
     bool operator==(const GraphKey& o) const {
+      const dip_track &a = track, &b = o.track;
       return z0 == o.z0 && target == o.target && mask == o.mask && out == o.out && slots == o.slots && adam_id == o.adam_id &&
-             adam_bind == o.adam_bind && sigma == o.sigma && seed == o.seed && lr == o.lr;
+             adam_bind == o.adam_bind && sigma == o.sigma && seed == o.seed && lr == o.lr && a.gt == b.gt &&
+             a.out_avg == b.out_avg && a.snapshot == b.snapshot && a.state == b.state && a.records == b.records &&
+             a.exp_weight == b.exp_weight && a.show_every == b.show_every && a.backtrack_db == b.backtrack_db;
     }
   };
   GraphKey gkey{};
@@ -1355,6 +1359,7 @@ struct dip_adam {
   int nblocks = 0;
   float** d_p = nullptr; const float** d_g = nullptr; float** d_m = nullptr; float** d_v = nullptr;
   int* d_blk_tensor = nullptr; int* d_blk_start = nullptr; int* d_numel = nullptr;
+  long long* d_off = nullptr;       // prefix sums of numel: tensor i's offset in a flat buffer (the tracker's snapshot)
   bool bound = false;
   unsigned long long id = 0;        // unique per dip_adam_create (graph cache key of dip_run_iterations)
   unsigned long long bind_gen = 0;  // bumped by dip_adam_bind (the captured k_adam reads the tables, not their addresses,
@@ -1562,8 +1567,10 @@ int dip_adam_create(int ntensors, const long long* numel, dip_adam** out) {
   a->n = ntensors;
   a->numel.assign(numel, numel + ntensors);
   std::vector<int> bt, bs, ne;
+  std::vector<long long> off;
   const int chunk = adam_chunk();
   for (int t = 0; t < ntensors; ++t) {
+    off.push_back(t == 0 ? 0 : off.back() + numel[t - 1]);
     ne.push_back((int)numel[t]);
     for (long long st = 0; st < numel[t]; st += chunk) { bt.push_back(t); bs.push_back((int)st); }
   }
@@ -1575,16 +1582,18 @@ int dip_adam_create(int ntensors, const long long* numel, dip_adam** out) {
   DIP_CUDA(cudaMalloc(&a->d_blk_tensor, bt.size() * sizeof(int)));
   DIP_CUDA(cudaMalloc(&a->d_blk_start, bs.size() * sizeof(int)));
   DIP_CUDA(cudaMalloc(&a->d_numel, ne.size() * sizeof(int)));
+  DIP_CUDA(cudaMalloc(&a->d_off, off.size() * sizeof(long long)));
   DIP_CUDA(cudaMemcpy(a->d_blk_tensor, bt.data(), bt.size() * sizeof(int), cudaMemcpyHostToDevice));
   DIP_CUDA(cudaMemcpy(a->d_blk_start, bs.data(), bs.size() * sizeof(int), cudaMemcpyHostToDevice));
   DIP_CUDA(cudaMemcpy(a->d_numel, ne.data(), ne.size() * sizeof(int), cudaMemcpyHostToDevice));
+  DIP_CUDA(cudaMemcpy(a->d_off, off.data(), off.size() * sizeof(long long), cudaMemcpyHostToDevice));
   *out = a;
   return 0;
 }
 void dip_adam_destroy(dip_adam* a) {
   if (!a) return;
   cudaFree(a->d_p); cudaFree(a->d_g); cudaFree(a->d_m); cudaFree(a->d_v);
-  cudaFree(a->d_blk_tensor); cudaFree(a->d_blk_start); cudaFree(a->d_numel);
+  cudaFree(a->d_blk_tensor); cudaFree(a->d_blk_start); cudaFree(a->d_numel); cudaFree(a->d_off);
   delete a;
 }
 int dip_adam_bind(dip_adam* a, void* const* p, void* const* g, void* const* m, void* const* v) {
@@ -1606,10 +1615,12 @@ int dip_adam_step(dip_adam* a, double lr, double beta1, double beta2, double eps
 }
 
 // One iteration of the lean closure: noise -> forward -> MSE -> backward -> Adam.  With it_dev != nullptr every
-// per-iteration scalar (Philox stream, loss slot, Adam step) comes from device counters, so the launch sequence is
-// identical for every iteration and can be replayed as a CUDA graph.
+// per-iteration scalar (Philox stream, loss slot, record slot, Adam step) comes from device counters, so the launch sequence
+// is identical for every iteration and can be replayed as a CUDA graph.  track != nullptr adds the tracker's two kernels
+// between the loss and the backward pass and steps Adam with its action; track->records is this call's first record.
 static int run_body(dip_plan* P, dip_adam* adam, const float* z0, const float* target, const float* mask, float sigma,
-                    uint64_t seed, int step_base, double lr, float* out, double* loss_slot, int* it_dev, cudaStream_t s) {
+                    uint64_t seed, int step_base, double lr, float* out, double* loss_slot, const dip_track* track, int* it_dev,
+                    cudaStream_t s) {
   const size_t nz = (size_t)P->H * P->W * P->desc.in_channels;
   const int hw = P->H * P->W;
   const float* zin = z0;
@@ -1647,29 +1658,65 @@ static int run_body(dip_plan* P, dip_adam* adam, const float* z0, const float* t
     ENQ(&runner, hbm(H_MSE, mask != nullptr), (3.0 * P->desc.out_channels + (mask != nullptr ? 1.0 : 0.0)) * hw * sizeof(float), s,
         launch_mse(P->out_saved, target, mask, P->desc.out_channels, hw, loss_slot, P->dout, slot_idx, s));
   }
+  TrackState* tstate = track != nullptr ? (TrackState*)track->state : nullptr;
+  if (track != nullptr) {
+    const int n = P->desc.out_channels * hw;
+    const bool gt = track->gt != nullptr;
+    ENQ(&runner, hbm(H_TRACK_OUT, gt), (gt ? 4.0 : 3.0) * n * sizeof(float), s,
+        launch_track_out(P->out_saved, (const float*)track->gt, (float*)track->out_avg, tstate, (float)track->exp_weight,
+                         (float)(1.0 - track->exp_weight), n, track->records, slot_idx, s));
+    ENQ(&runner, hbm(H_TRACK_DECIDE, 0), (kTrackRecord + 1.0) * sizeof(double) + 2.0 * sizeof(TrackState), s,
+        launch_track_decide(loss_slot, track->records, tstate, track->show_every, track->backtrack_db, gt, slot_idx, s));
+  }
   DIP_CHECK(plan_backward(P, P->dout, s));
   if (!adam->bound) return fail("dip_run_iterations: adam not bound");
   AdamTable t{adam->d_p, adam->d_g, adam->d_m, adam->d_v, adam->d_blk_tensor, adam->d_blk_start, adam->d_numel, adam->nblocks};
   {
     double np_ = 0; for (long long n : adam->numel) np_ += (double)n;
-    ENQ(&runner, hbm(H_ADAM, 0), 7.0 * np_ * sizeof(float), s, launch_adam(t, lr, 0.9, 0.999, 1e-8, step_base + 1, it_dev, s));
+    if (track == nullptr)
+      ENQ(&runner, hbm(H_ADAM, 0), 7.0 * np_ * sizeof(float), s, launch_adam(t, lr, 0.9, 0.999, 1e-8, step_base + 1, it_dev, s));
+    else   // + the snapshot write of a save
+      ENQ(&runner, hbm(H_ADAM_TRACK, 0), 8.0 * np_ * sizeof(float), s,
+          launch_adam_track(t, lr, 0.9, 0.999, 1e-8, step_base + 1, it_dev, AdamTrack{tstate, (float*)track->snapshot, adam->d_off}, s));
   }
   if (it_dev != nullptr) launch_advance(it_dev, s);
   DIP_CUDA(cudaGetLastError());
   return 0;
 }
 
-int dip_run_iterations(dip_plan* P, dip_adam* adam, const void* z0, const void* target, const void* mask, float sigma,
-                       uint64_t seed, int step0, int iters, double lr, void* out, double* loss_hist, dip_stream_t stream) {
+size_t dip_track_state_bytes(void) { return sizeof(TrackState); }
+
+static int check_track(const dip_track* t) {
+  if (!(t->exp_weight >= 0.0 && t->exp_weight < 1.0))
+    return fail("dip_run_iterations_tracked: exp_weight must be in [0, 1), got " + std::to_string(t->exp_weight));
+  if (t->show_every < 0) return fail("dip_run_iterations_tracked: show_every must be >= 0, got " + std::to_string(t->show_every));
+  if (t->backtrack_db != t->backtrack_db) return fail("dip_run_iterations_tracked: backtrack_db is NaN");
+  if (t->out_avg == nullptr) return fail("dip_run_iterations_tracked: out_avg is NULL");
+  if (t->snapshot == nullptr) return fail("dip_run_iterations_tracked: snapshot is NULL");
+  if (t->state == nullptr) return fail("dip_run_iterations_tracked: state is NULL");
+  if (t->records == nullptr) return fail("dip_run_iterations_tracked: records is NULL");
+  return 0;
+}
+
+int dip_run_iterations_tracked(dip_plan* P, dip_adam* adam, const void* z0, const void* target, const void* mask, float sigma,
+                               uint64_t seed, int step0, int iters, double lr, void* out, double* loss_hist,
+                               const dip_track* track, dip_stream_t stream) {
   cudaStream_t s = (cudaStream_t)stream;
+  if (track != nullptr) DIP_CHECK(check_track(track));
   if (iters <= 0) return 0;
   const bool use_graph = !P->timer.on && getenv("DIP_NO_GRAPH") == nullptr;
   if (!use_graph) {
     for (int i = 0; i < iters; ++i) {
       double* lp = loss_hist != nullptr ? loss_hist + i : P->loss_ring;
       DIP_CUDA(cudaMemsetAsync(lp, 0, sizeof(double), s));
+      dip_track ti;
+      if (track != nullptr) {
+        ti = *track;
+        ti.records = track->records + (size_t)kTrackRecord * i;
+        DIP_CUDA(cudaMemsetAsync(ti.records, 0, kTrackRecord * sizeof(double), s));
+      }
       DIP_CHECK(run_body(P, adam, (const float*)z0, (const float*)target, (const float*)mask, sigma, seed, step0 + i, lr,
-                         (float*)out, lp, nullptr, s));
+                         (float*)out, lp, track != nullptr ? &ti : nullptr, nullptr, s));
     }
     return 0;
   }
@@ -1677,7 +1724,10 @@ int dip_run_iterations(dip_plan* P, dip_adam* adam, const void* z0, const void* 
     // internal ring too small: split the call
     for (int done = 0; done < iters; done += dip_plan::kLossRing) {
       const int n = iters - done < dip_plan::kLossRing ? iters - done : dip_plan::kLossRing;
-      DIP_CHECK(dip_run_iterations(P, adam, z0, target, mask, sigma, seed, step0 + done, n, lr, out, nullptr, stream));
+      dip_track tc;
+      if (track != nullptr) { tc = *track; tc.records = track->records + (size_t)kTrackRecord * done; }
+      DIP_CHECK(dip_run_iterations_tracked(P, adam, z0, target, mask, sigma, seed, step0 + done, n, lr, out, nullptr,
+                                           track != nullptr ? &tc : nullptr, stream));
     }
     return 0;
   }
@@ -1690,21 +1740,28 @@ int dip_run_iterations(dip_plan* P, dip_adam* adam, const void* z0, const void* 
   dip_plan::GraphKey key;
   key.z0 = z0; key.target = target; key.mask = mask; key.out = out; key.slots = slots;
   key.adam_id = adam->id; key.adam_bind = adam->bind_gen; key.sigma = sigma; key.seed = seed; key.lr = lr;
+  if (track != nullptr) key.track = *track;
   if (P->gexec == nullptr || !(key == P->gkey)) {
     if (P->gexec != nullptr) { cudaGraphExecDestroy(P->gexec); P->gexec = nullptr; }
     DIP_CHECK(capture_graph(gs, &P->gexec, [&](cudaStream_t cs) {
       return run_body(P, adam, (const float*)z0, (const float*)target, (const float*)mask, sigma, seed, 0, lr, (float*)out, slots,
-                      P->it_dev, cs);
+                      track, P->it_dev, cs);
     }));
     P->gkey = key;
   }
   const int init[2] = {step0, 0};
   DIP_CUDA(cudaMemcpyAsync(P->it_dev, init, sizeof init, cudaMemcpyHostToDevice, gs));
   DIP_CUDA(cudaMemsetAsync(slots, 0, (size_t)iters * sizeof(double), gs));
+  if (track != nullptr) DIP_CUDA(cudaMemsetAsync(track->records, 0, (size_t)iters * kTrackRecord * sizeof(double), gs));
   for (int i = 0; i < iters; ++i) DIP_CUDA(cudaGraphLaunch(P->gexec, gs));
   DIP_CUDA(cudaEventRecord(P->gev_out, gs));
   DIP_CUDA(cudaStreamWaitEvent(s, P->gev_out, 0));
   return 0;
+}
+
+int dip_run_iterations(dip_plan* P, dip_adam* adam, const void* z0, const void* target, const void* mask, float sigma,
+                       uint64_t seed, int step0, int iters, double lr, void* out, double* loss_hist, dip_stream_t stream) {
+  return dip_run_iterations_tracked(P, adam, z0, target, mask, sigma, seed, step0, iters, lr, out, loss_hist, nullptr, stream);
 }
 
 int dip_input_grad(dip_plan* P, void* dz, dip_stream_t stream) {

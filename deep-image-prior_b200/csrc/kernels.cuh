@@ -245,6 +245,38 @@ void launch_adam(AdamTable t, double lr, double b1, double b2, double eps, int s
                  cudaStream_t s);
 int adam_chunk();
 
+// Denoising-closure tracker (denoising.ipynb c10:8-52, dip_track in include/dip.h) ---------------------------------------
+// Persistent state; all zero = the notebook's initial globals (i = 0, out_avg = None, last_net = None, psrn_noisy_last = 0).
+struct TrackState {
+  double psnr_last;   // psrn_noisy_last
+  int i;              // the notebook's iteration counter (not advanced by a restore)
+  int action;         // this iteration's decision, read by the tracked Adam step: kTrack*
+  int has_avg;        // out_avg holds an average (0: the next output is copied)
+  int has_snapshot;   // the snapshot holds parameters (last_net is not None)
+  int fallbacks;      // restores so far
+  int unused;
+};
+enum { kTrackNone = 0, kTrackSaved = 1, kTrackRestored = 2 };
+static constexpr int kTrackRecord = 6;   // doubles per iteration: loss, psnr_target, psnr_gt, psnr_gt_sm, i, action
+// out_avg = out (first tracked iteration) or fl(fl(out_avg * w_avg) + fl(out * w_out)); with gt != null the two fp64 sums
+// mean((out - gt)^2), mean((out_avg - gt)^2) are accumulated into rec[slot][2], rec[slot][3] with k_mse's reduction
+// (slot = *it_dev if it_dev != null else 0; the slot must be zero)
+void launch_track_out(const float* out, const float* gt, float* out_avg, const TrackState* st, float w_avg, float w_out,
+                      int n, double* rec, const int* it_dev, cudaStream_t s);
+// one warp: rec[slot] = {loss[slot], PSNRs of the loss and of the two sums (NaN without gt), i, action}; applies the
+// back-tracking rule and updates *st
+void launch_track_decide(const double* loss, double* rec, TrackState* st, int show_every, double backtrack_db, int has_gt,
+                         const int* it_dev, cudaStream_t s);
+// Adam with the tracker's action: st->action == kTrackRestored steps from the snapshot instead of p; kTrackSaved stores the
+// p it read into the snapshot.  snapshot: one flat buffer, tensor i at off[i] (the tensors' numel prefix sums).
+struct AdamTrack {
+  const TrackState* st;
+  float* snapshot;
+  const long long* off;
+};
+void launch_adam_track(AdamTable t, double lr, double b1, double b2, double eps, int step, const int* it_dev, AdamTrack tr,
+                       cudaStream_t s);
+
 // SIMT fp32 reference convolutions (exact-fp32 mode) ---------------------------------------------------
 struct SimtConvArgs {
   const float* A; int a_h, a_w, a_ld, a_c;       // input NHWC (rows, cols, stride, valid channels)

@@ -15,6 +15,7 @@
 #include "kernels.cuh"
 
 #include <cuda_bf16.h>
+#include <math_constants.h>
 #include <math.h>
 #include <stdlib.h>
 
@@ -1513,12 +1514,18 @@ void launch_advance(int* it_dev, cudaStream_t s) { launch_k(k_advance, dim3(1), 
 // Arithmetic order follows torch.optim.Adam (single-tensor path): m = lerp(m, g, 1-b1); v = v*b2 + (1-b2) g^2;
 // p -= (lr/bc1) * m / (sqrt(v)/sqrt(bc2) + eps).  Bias corrections are evaluated in fp64 on the device so that the
 // step number can come from a device counter (CUDA-graph replay).
+// kTrack: the tracker's action (AdamTrack) selects where p comes from and whether it is saved; the untracked instantiation
+// never reads `tr`.
 static constexpr int kAdamChunk = 2048;
-__global__ void k_adam(AdamTable t, double lr, double b1, double b2, double eps, int step, const int* __restrict__ it_dev) {
+template <bool kTrack>
+__global__ void k_adam(AdamTable t, double lr, double b1, double b2, double eps, int step, const int* __restrict__ it_dev,
+                       AdamTrack tr) {
   pdl_enter();
   __shared__ float s_step_size, s_bc2_sqrt;
+  __shared__ int s_action;
   if (threadIdx.x == 0) {
     const int st = step + (it_dev != nullptr ? *it_dev : 0);
+    if (kTrack) s_action = tr.st->action;
     const double bc1 = 1.0 - pow(b1, static_cast<double>(st));
     const double bc2 = 1.0 - pow(b2, static_cast<double>(st));
     s_step_size = static_cast<float>(lr / bc1);
@@ -1536,6 +1543,22 @@ __global__ void k_adam(AdamTable t, double lr, double b1, double b2, double eps,
   float* __restrict__ m = t.m[ti];
   float* __restrict__ v = t.v[ti];
   const int end = min(start + kAdamChunk, n);
+  if (!kTrack) {
+    for (int i = start + threadIdx.x; i < end; i += blockDim.x) {
+      const float gi = g[i];
+      float mi = m[i];
+      mi = mi + (gi - mi) * w1;
+      const float vi = v[i] * fb2 + w2 * gi * gi;
+      m[i] = mi;
+      v[i] = vi;
+      const float denom = sqrtf(vi) / bc2_sqrt + feps;
+      p[i] = p[i] - step_size * (mi / denom);
+    }
+    return;
+  }
+  const int action = s_action;
+  float* __restrict__ snap = tr.snapshot + tr.off[ti];
+  const float* src = action == kTrackRestored ? snap : p;
   for (int i = start + threadIdx.x; i < end; i += blockDim.x) {
     const float gi = g[i];
     float mi = m[i];
@@ -1544,11 +1567,107 @@ __global__ void k_adam(AdamTable t, double lr, double b1, double b2, double eps,
     m[i] = mi;
     v[i] = vi;
     const float denom = sqrtf(vi) / bc2_sqrt + feps;
-    p[i] = p[i] - step_size * (mi / denom);
+    const float pi = src[i];
+    if (action == kTrackSaved) snap[i] = pi;
+    p[i] = pi - step_size * (mi / denom);
   }
 }
 void launch_adam(AdamTable t, double lr, double b1, double b2, double eps, int step, const int* it_dev, cudaStream_t s) {
-  launch_k(k_adam, dim3(t.nblocks), dim3(256), 0, s, 1, t, lr, b1, b2, eps, step, it_dev);
+  launch_k(k_adam<false>, dim3(t.nblocks), dim3(256), 0, s, 1, t, lr, b1, b2, eps, step, it_dev, AdamTrack{});
+}
+void launch_adam_track(AdamTable t, double lr, double b1, double b2, double eps, int step, const int* it_dev, AdamTrack tr,
+                       cudaStream_t s) {
+  launch_k(k_adam<true>, dim3(t.nblocks), dim3(256), 0, s, 1, t, lr, b1, b2, eps, step, it_dev, tr);
+}
+
+// ------------------------------------------------------------------------------------------------ closure tracker
+// denoising.ipynb c10:8-52 inside the captured step.  k_track_out: the EMA in torch's rounding (`out_avg * w + out * (1 - w)`
+// on fp32 CUDA tensors: each scalar rounded to fp32, three separately rounded operations) and the two ground-truth MSEs
+// with k_mse's reduction, so that they do not depend on block order either.
+__global__ void k_track_out(const float* __restrict__ out, const float* __restrict__ gt, float* __restrict__ avg,
+                            const TrackState* __restrict__ st, float w_avg, float w_out, int n, double* __restrict__ rec,
+                            const int* __restrict__ it_dev) {
+  pdl_enter();
+  const bool first = st->has_avg == 0;
+  const float inv_n = 1.f / static_cast<float>(n);
+  float acc_out = 0.f, acc_avg = 0.f;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const float o = out[i];
+    const float a = first ? o : __fadd_rn(__fmul_rn(avg[i], w_avg), __fmul_rn(o, w_out));
+    avg[i] = a;
+    if (gt != nullptr) {
+      const float g = gt[i];
+      const float d0 = o - g, d1 = a - g;
+      acc_out = fmaf(d0, d0, acc_out);
+      acc_avg = fmaf(d1, d1, acc_avg);
+    }
+  }
+  if (gt == nullptr) return;
+  __shared__ float red[2][32];
+  for (int o = 16; o > 0; o >>= 1) {
+    acc_out += __shfl_xor_sync(0xffffffffu, acc_out, o);
+    acc_avg += __shfl_xor_sync(0xffffffffu, acc_avg, o);
+  }
+  if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = acc_out; red[1][threadIdx.x >> 5] = acc_avg; }
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    float t0 = threadIdx.x < (blockDim.x >> 5) ? red[0][threadIdx.x] : 0.f;
+    float t1 = threadIdx.x < (blockDim.x >> 5) ? red[1][threadIdx.x] : 0.f;
+    for (int o = 16; o > 0; o >>= 1) {
+      t0 += __shfl_xor_sync(0xffffffffu, t0, o);
+      t1 += __shfl_xor_sync(0xffffffffu, t1, o);
+    }
+    if (threadIdx.x == 0) {   // as k_mse: each block's term rounded to a multiple of 2^-48
+      double* r = rec + kTrackRecord * (it_dev != nullptr ? *it_dev : 0);
+      atomicAdd(r + 2, ldexp(rint(ldexp(static_cast<double>(t0) * static_cast<double>(inv_n), 48)), -48));
+      atomicAdd(r + 3, ldexp(rint(ldexp(static_cast<double>(t1) * static_cast<double>(inv_n), 48)), -48));
+    }
+  }
+}
+void launch_track_out(const float* out, const float* gt, float* out_avg, const TrackState* st, float w_avg, float w_out,
+                      int n, double* rec, const int* it_dev, cudaStream_t s) {
+  int blocks = (n + 255) / 256;   // launch_mse's grid: the same per-thread terms
+  if (blocks > kNumSms * 4) blocks = kNumSms * 4;
+  launch_k(k_track_out, dim3(blocks), dim3(256), 0, s, 1, out, gt, out_avg, st, w_avg, w_out, n, rec, it_dev);
+}
+// c10:41-52: PSNRs (skimage compare_psnr, data range 1) of the iteration's loss and sums, then the back-tracking rule.
+// A restore leaves i and psnr_last alone; a drop with no snapshot yet saves.
+__global__ void k_track_decide(const double* __restrict__ loss, double* __restrict__ rec, TrackState* __restrict__ st,
+                               int show_every, double backtrack_db, int has_gt, const int* __restrict__ it_dev) {
+  pdl_enter();
+  if (threadIdx.x != 0) return;
+  const int slot = it_dev != nullptr ? *it_dev : 0;
+  double* r = rec + kTrackRecord * slot;
+  const double l = loss[slot];
+  const double psnr = -10.0 * log10(l);
+  r[0] = l;
+  r[1] = psnr;
+  r[2] = has_gt ? -10.0 * log10(r[2]) : CUDART_NAN;
+  r[3] = has_gt ? -10.0 * log10(r[3]) : CUDART_NAN;
+  TrackState x = *st;
+  r[4] = static_cast<double>(x.i);
+  int action = kTrackNone;
+  if (show_every > 0 && x.i % show_every != 0) {
+    if (psnr - x.psnr_last < -backtrack_db && x.has_snapshot) {
+      action = kTrackRestored;
+      x.fallbacks += 1;
+    } else {
+      action = kTrackSaved;
+      x.has_snapshot = 1;
+      x.psnr_last = psnr;
+      x.i += 1;
+    }
+  } else {
+    x.i += 1;
+  }
+  x.action = action;
+  x.has_avg = 1;
+  *st = x;
+  r[5] = static_cast<double>(action);
+}
+void launch_track_decide(const double* loss, double* rec, TrackState* st, int show_every, double backtrack_db, int has_gt,
+                         const int* it_dev, cudaStream_t s) {
+  launch_k(k_track_decide, dim3(1), dim3(32), 0, s, 1, loss, rec, st, show_every, backtrack_db, has_gt, it_dev);
 }
 int adam_chunk() { return kAdamChunk; }
 

@@ -48,6 +48,17 @@ class NetDesc(ctypes.Structure):
     ]
 
 
+class Track(ctypes.Structure):
+    """dip_track (include/dip.h): the denoising closure's EMA, PSNRs and back-tracking inside the runner"""
+    _fields_ = [("gt", ctypes.c_void_p), ("out_avg", ctypes.c_void_p), ("snapshot", ctypes.c_void_p),
+                ("state", ctypes.c_void_p), ("records", ctypes.c_void_p), ("exp_weight", ctypes.c_double),
+                ("show_every", ctypes.c_int), ("backtrack_db", ctypes.c_double)]
+
+
+RECORD = 6                     # doubles per tracked iteration: loss, psnr_target, psnr_gt, psnr_gt_sm, i, action
+ACTION_NONE, ACTION_SAVED, ACTION_RESTORED = 0, 1, 2
+
+
 class PlanOpts(ctypes.Structure):
     """dip_plan_opts (include/dip.h): PlanOpts(pad_mode, act_fun); a field left out is 0 (reflection, LeakyReLU)"""
     _fields_ = [("pad_mode", ctypes.c_int), ("act_fun", ctypes.c_int)]
@@ -64,6 +75,7 @@ ABI_SYMBOLS = [
     "dip_op_conv_dgrad", "dip_op_conv_wgrad", "dip_op_conv_dgrad_s2",
     "dip_lanczos_down_out_size", "dip_lanczos_down_fwd", "dip_lanczos_down_bwd", "dip_plan_set_downsampler",
     "dip_input_grad", "dip_plan_workspace_bytes_opts", "dip_plan_create_opts",
+    "dip_track_state_bytes", "dip_run_iterations_tracked",
 ]
 
 
@@ -116,6 +128,8 @@ def lib():
     L.dip_adam_bind.argtypes = [vp, pvp, pvp, pvp, pvp]
     L.dip_adam_step.argtypes = [vp, f64, f64, f64, f64, i32, vp]
     L.dip_run_iterations.argtypes = [vp, vp, vp, vp, vp, f32, u64, i32, i32, f64, vp, vp, vp]
+    L.dip_track_state_bytes.restype = sz
+    L.dip_run_iterations_tracked.argtypes = [vp, vp, vp, vp, vp, f32, u64, i32, i32, f64, vp, vp, ctypes.POINTER(Track), vp]
     L.dip_plan_buffer.argtypes = [vp, ctypes.c_char_p, pvp, ctypes.POINTER(i32)]
     L.dip_plan_num_launches.argtypes = [vp, ctypes.POINTER(i32), ctypes.POINTER(i32)]
     L.dip_plan_set_timing.argtypes = [vp, i32]
@@ -362,17 +376,72 @@ class FusedAdam:
                                       _stream()))
 
 
-def run_iterations(plan, adam, z0, target, mask, sigma, seed, iters, lr, out=None, loss_hist=None):
+class Tracker:
+    """State of the denoising closure (denoising.ipynb c10:8-52) that run_iterations(track=...) keeps on the device: the
+    EMA `out_avg`, the parameter snapshot (`last_net`, flat in the Adam tensors' order like FusedAdam.m_flat) and the
+    back-tracking state.  gt: the clean image (psnr_gt / psnr_gt_sm; NaN without it).  Defaults are c10's."""
+
+    def __init__(self, adam, out_shape, gt=None, exp_weight=0.99, show_every=100, backtrack_db=5.0):
+        dev = adam.params[0].device
+        self.adam = adam
+        self.gt = None if gt is None else gt.detach().to(device=dev, dtype=torch.float32).contiguous()
+        if self.gt is not None and tuple(self.gt.shape) != tuple(out_shape):
+            raise ValueError("dip-b200: Tracker gt has shape %s, the output %s" % (tuple(self.gt.shape), tuple(out_shape)))
+        self.exp_weight, self.show_every, self.backtrack_db = float(exp_weight), int(show_every), float(backtrack_db)
+        self.out_avg = torch.zeros(out_shape, dtype=torch.float32, device=dev)
+        self.snapshot = torch.zeros(adam.m_flat.numel(), dtype=torch.float32, device=dev)
+        self.state = torch.zeros(lib().dip_track_state_bytes(), dtype=torch.uint8, device=dev)
+
+    def reset(self):
+        """back to the notebook's initial globals: i = 0, out_avg = None, last_net = None, psrn_noisy_last = 0"""
+        self.state.zero_()
+
+    def _state(self):
+        s = self.state.cpu()
+        return s[:8].view(torch.float64).item(), s[8:].view(torch.int32).tolist()   # TrackState (kernels.cuh)
+
+    @property
+    def i(self):
+        return self._state()[1][0]
+
+    @property
+    def fallbacks(self):
+        return self._state()[1][4]
+
+    @property
+    def psnr_last(self):
+        return self._state()[0]
+
+    def struct(self, records):
+        return Track(_ptr(self.gt).value, self.out_avg.data_ptr(), self.snapshot.data_ptr(), self.state.data_ptr(),
+                     records.data_ptr(), self.exp_weight, self.show_every, self.backtrack_db)
+
+
+def run_iterations(plan, adam, z0, target, mask, sigma, seed, iters, lr, out=None, loss_hist=None, track=None,
+                   records=None):
     """Closure-free device loop (dip_run_iterations): noise -> forward -> MSE -> backward -> Adam, `iters` times.
     The device loop's Adam step uses torch's default betas and eps; an optimiser with others is refused, not stepped
-    with the defaults."""
+    with the defaults.  track: a Tracker of `adam`, which then needs `records`, an fp64 CUDA tensor of iters x 6
+    (dip_run_iterations_tracked)."""
     if tuple(adam.betas) != (0.9, 0.999):
         raise ValueError("dip-b200: run_iterations steps Adam with betas (0.9, 0.999); adam.betas is %r" % (adam.betas,))
     if adam.eps != 1e-8:
         raise ValueError("dip-b200: run_iterations steps Adam with eps 1e-8; adam.eps is %r" % (adam.eps,))
+    tr = None
+    if track is not None:
+        if track.adam is not adam:
+            raise ValueError("dip-b200: run_iterations: the Tracker belongs to another optimiser")
+        if (records is None or not records.is_cuda or records.dtype != torch.float64 or not records.is_contiguous()
+                or records.numel() < RECORD * iters):
+            raise ValueError("dip-b200: run_iterations(track=...) needs records, a contiguous fp64 CUDA tensor of >= %d x %d"
+                             % (iters, RECORD))
+        tr = ctypes.byref(track.struct(records))
+    elif records is not None:
+        raise ValueError("dip-b200: run_iterations: records without a Tracker")
     with torch.cuda.device(plan.device):
-        check(lib().dip_run_iterations(plan.h, adam.h, _ptr(z0), _ptr(target), _ptr(mask), float(sigma), int(seed),
-                                       adam.step_count, int(iters), float(lr), _ptr(out), _ptr(loss_hist), _stream()))
+        check(lib().dip_run_iterations_tracked(plan.h, adam.h, _ptr(z0), _ptr(target), _ptr(mask), float(sigma), int(seed),
+                                               adam.step_count, int(iters), float(lr), _ptr(out), _ptr(loss_hist), tr,
+                                               _stream()))
     adam.step_count += iters
 
 

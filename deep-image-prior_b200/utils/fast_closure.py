@@ -15,6 +15,14 @@ good parameters when PSNR_noisy drops by more than 5 dB -- but keeps the quantit
     closure = DenoisingClosure(net, net_input, img_noisy_torch, img_torch, reg_noise_std=1. / 30, exp_weight=0.99)
     optimize('adam', get_params('net', net, net_input), closure, LR, num_iter)
     closure.history  ->  [(loss, psnr_noisy, psnr_gt, psnr_gt_sm), ...];  closure.out_avg  ->  the smoothed output
+
+DenoisingRun keeps the same logic inside the device runner (dip_run_iterations_tracked): the EMA, the PSNRs, the
+back-tracking decision and the parameter snapshot / restore are made on the device within each replayed step, so a run of
+any length needs one read-back at its end instead of one per iteration:
+
+    run = DenoisingRun(net, net_input, img_noisy_torch, img_torch, reg_noise_std=1. / 30, LR=0.01)
+    run.run(num_iter)
+    run.history  ->  [(loss, psnr_noisy, psnr_gt, psnr_gt_sm, action), ...];  run.out_avg, run.fallbacks, run.i
 """
 import math
 
@@ -100,3 +108,64 @@ class DenoisingClosure:
             self.psrn_noisy_last = psrn_noisy
         self.i += 1
         return total_loss
+
+
+class DenoisingRun:
+    """The denoising.ipynb c10 closure in the device runner: noise -> forward -> MSE -> EMA, PSNRs, back-tracking ->
+    backward -> Adam, one captured CUDA graph per iteration.  Same arguments as DenoisingClosure plus the Adam learning
+    rate `LR` and the noise `seed` (Philox stream, offset = Adam step); `mse` may only be None or an nn.MSELoss, since the
+    runner takes the MSE itself, and a host callback cannot run inside the device loop.  backtrack_db: the drop of
+    psrn_noisy that restores the last good parameters (5 dB in c10:42).
+
+    history rows: (loss, psnr_noisy, psnr_gt, psnr_gt_sm, action) with action 0 none, 1 saved, 2 restored.  Without
+    img_torch the ground-truth PSNRs are taken against the noisy image, as DenoisingClosure does."""
+
+    def __init__(self, net, net_input, img_noisy_torch, img_torch=None, reg_noise_std=1. / 30, exp_weight=0.99,
+                 show_every=100, mse=None, on_show=None, LR=0.01, seed=0, backtrack_db=5.0):
+        import dip_engine as de
+        if mse is not None and type(mse) is not torch.nn.MSELoss:
+            raise ValueError("dip-b200: DenoisingRun takes the loss as the runner's MSE; mse must be None or nn.MSELoss()")
+        if on_show is not None:
+            raise ValueError("dip-b200: DenoisingRun cannot call on_show from inside the device loop; "
+                             "read out_avg between run() calls")
+        if getattr(net, "_dip_spec", None) is None:
+            raise ValueError("dip-b200: DenoisingRun needs a network that runs on the engine (%s)"
+                             % getattr(net, "_dip_why", "not a models.skip network"))
+        if net_input.requires_grad:
+            raise ValueError("dip-b200: DenoisingRun does not optimise the network input (OPT_OVER 'net,input')")
+        self.z = net_input.detach().contiguous()
+        self.plan, params = net._engine_state(self.z)
+        if self.plan.desc.input_grad:
+            raise ValueError("dip-b200: DenoisingRun does not run plans with input_grad")
+        self.net, self.LR, self.seed, self.reg_noise_std = net, float(LR), int(seed), float(reg_noise_std)
+        self.target = img_noisy_torch.detach().to(self.z.device, torch.float32).contiguous()
+        gt = img_torch if img_torch is not None else img_noisy_torch
+        self.adam = de.FusedAdam(params, lr=self.LR)
+        self.adam._bind(net._dip_grad_views)
+        self.out = torch.empty((1, self.plan.desc.out_channels, self.plan.H, self.plan.W), dtype=torch.float32,
+                               device=self.z.device)
+        self.tracker = de.Tracker(self.adam, tuple(self.out.shape), gt=gt, exp_weight=exp_weight, show_every=show_every,
+                                  backtrack_db=backtrack_db)
+        self.i = 0
+        self.fallbacks = 0
+        self.history = []
+
+    @property
+    def out_avg(self):
+        return self.tracker.out_avg
+
+    def run(self, num_iter):
+        """num_iter iterations in one runner call, then one read-back of their records"""
+        import dip_engine as de
+        if num_iter <= 0:
+            return self.history
+        records = torch.empty((num_iter, de.RECORD), dtype=torch.float64, device=self.z.device)
+        de.run_iterations(self.plan, self.adam, self.z, self.target, None, self.reg_noise_std, self.seed, num_iter, self.LR,
+                          out=self.out, track=self.tracker, records=records)
+        rows = records.cpu().tolist()
+        for loss, psnr_noisy, psnr_gt, psnr_gt_sm, i, action in rows:
+            self.history.append((loss, psnr_noisy, psnr_gt, psnr_gt_sm, int(action)))
+            self.fallbacks += int(action) == de.ACTION_RESTORED
+        last = rows[-1]
+        self.i = int(last[4]) + (int(last[5]) != de.ACTION_RESTORED)
+        return self.history

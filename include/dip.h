@@ -140,6 +140,39 @@ int dip_run_iterations(dip_plan* plan, dip_adam* adam, const void* z0, const voi
                        float sigma, uint64_t seed, int step0, int iters, double lr, void* out, double* loss_hist,
                        dip_stream_t stream);
 
+/* ---- the runner with the rest of the denoising closure (denoising.ipynb c10:8-56) on the device: every iteration, after
+ *      the loss and before the Adam step,
+ *        1. out_avg = out (first tracked iteration), else out_avg * exp_weight + out * (1 - exp_weight) in torch's fp32
+ *           rounding (each scalar rounded to fp32, three separately rounded operations);
+ *        2. psnr_target = -10 log10(loss) (c10's psrn_noisy; psrn_masked / psnr_LR for inpainting / super-resolution),
+ *           psnr_gt = -10 log10(mean((out - gt)^2)), psnr_gt_sm = the same for the updated out_avg, all in fp64
+ *           (skimage compare_psnr, data range 1; unmasked; NaN without gt);
+ *        3. back-tracking (c10:41-52) when show_every > 0 and i % show_every != 0: if psnr_target - psnr_last <
+ *           -backtrack_db and a snapshot exists, the Adam step starts from the snapshot instead of the parameters (m, v and
+ *           the step advance with this iteration's gradient), i stays, fallbacks += 1; otherwise the snapshot becomes the
+ *           parameters this iteration's forward used, psnr_last = psnr_target, i += 1.  Elsewhere only i += 1.
+ *           BatchNorm running statistics are not restored (the notebook does not restore them either);
+ *        4. records[iteration] = {loss, psnr_target, psnr_gt, psnr_gt_sm, i before this iteration, action}, action
+ *           0 none, 1 saved, 2 restored.
+ *      The state persists across calls; all zero = the notebook's initial globals (i = 0, out_avg = None, last_net = None,
+ *      psrn_noisy_last = 0). */
+typedef struct {
+  const void* gt;        /* [C_out][H][W] clean image, or NULL (psnr_gt / psnr_gt_sm = NaN)                        */
+  void* out_avg;         /* [C_out][H][W] fp32: the EMA                                                            */
+  void* snapshot;        /* fp32, sum of the Adam tensors' numel, in their order                                   */
+  void* state;           /* dip_track_state_bytes() bytes; all zero = the notebook's initial globals               */
+  double* records;       /* [iters][6], see above                                                                  */
+  double exp_weight;     /* in [0, 1); 0.99 in denoising.ipynb c10 (double: the rounding of 1 - exp_weight is torch's) */
+  int show_every;        /* >= 0; 0 = no back-tracking                                                             */
+  double backtrack_db;   /* 5 in denoising.ipynb c10:42                                                            */
+} dip_track;
+size_t dip_track_state_bytes(void);
+/* dip_run_iterations with the tracker above; track == NULL is dip_run_iterations.  Invalid fields are refused before
+ * anything is launched (dip_last_error() names the field). */
+int dip_run_iterations_tracked(dip_plan* plan, dip_adam* adam, const void* z0, const void* target, const void* mask,
+                               float sigma, uint64_t seed, int step0, int iters, double lr, void* out, double* loss_hist,
+                               const dip_track* track, dip_stream_t stream);
+
 /* ---- test / profiling access to internal NHWC buffers: name e.g. "L0.raw_u"; dims = {rows, cols, ld, channels} */
 int dip_plan_buffer(const dip_plan* plan, const char* name, void** ptr, int* dims4);
 int dip_plan_num_launches(const dip_plan* plan, int* fwd, int* bwd);
