@@ -6,13 +6,16 @@
 
 namespace dip {
 
-// D[y][x][n] = bias[n] + sum_{r,s,c} A[y*stride+offy+r][x*stride+offx+s][c] * Wp[tap][n][c]   (OOB reads = 0)
+// D[y][x][n] = bias[n] + sum_{r,s,c} A'[y*stride+offy+r][x*stride+offx+s][c] * Wp[tap][n][c]   (OOB reads = 0), where
+// A' is A dilated by `dil`: A'[iy][ix] = A[iy / dil][ix / dil] when dil divides both, else 0.  Dilation 2 with stride 1
+// is the input gradient of a stride-2 conv, read from dY at its own resolution.
 // Block: 16 consecutive output pixels of one row x all n_rows outputs (thread = output channel).
 static constexpr int kSimtPx = 16;
 __global__ void __launch_bounds__(160) k_simt_conv(SimtConvArgs a) {
   pdl_enter();
   __shared__ __align__(16) float As[32][kSimtPx];  // [c][px]
   __shared__ float Ws[160][33];                    // [n][c] (+1 pad)
+  const int sh = a.dil >> 1;                       // dil = 1 or 2: log2(dil), and the mask of an odd coordinate
   const int n = threadIdx.x;
   const int xb = blockIdx.x * kSimtPx;
   const int y = blockIdx.y;
@@ -29,8 +32,8 @@ __global__ void __launch_bounds__(160) k_simt_conv(SimtConvArgs a) {
           const int c = i & 31, px = i >> 5;
           const int ix = (xb + px) * a.stride + a.offx + s;
           float v = 0.f;
-          if (iy >= 0 && iy < a.a_h && ix >= 0 && ix < a.a_w && c0 + c < a.a_c)
-            v = a.A[(static_cast<long long>(iy) * a.a_w + ix) * a.a_ld + c0 + c];
+          if (iy >= 0 && (iy >> sh) < a.a_h && ix >= 0 && (ix >> sh) < a.a_w && ((iy | ix) & sh) == 0 && c0 + c < a.a_c)
+            v = a.A[(static_cast<long long>(iy >> sh) * a.a_w + (ix >> sh)) * a.a_ld + c0 + c];
           As[c][px] = v;
         }
         for (int i = threadIdx.x; i < a.n_rows * 32; i += blockDim.x) {

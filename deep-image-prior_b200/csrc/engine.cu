@@ -189,7 +189,7 @@ struct PackEntry {
   const float* w; float* dst_f; float* dst_d;
   int N, C, k, rot, n_rows, c_pad, c_rows;
   int Ctot, coff;   // weight has Ctot input channels; this entry packs engine channels [coff, coff + C)
-  int s2;           // dgrad pack of a stride-2 3x3 conv: taps in sub-pixel phase order (kS2Taps), not flipped
+  int s2;           // tensor-core dgrad pack of a stride-2 3x3 conv: taps in sub-pixel phase order (kS2Taps), not flipped
   int bf16;         // packs hold bf16 (same buffers); the fprop pack then has rows of c_pad16 (multiple of 64) channels
   int c_pad16;
   int n_pad;        // columns of the dgrad pack: N rounded up to 32 (bf16: to 64)
@@ -288,8 +288,9 @@ struct ConvOp {
   const float* dy = nullptr;
   // dgrad: dY -> dg_out [dg_out_h][dg_out_w][C]
   bool has_dgrad = false;
-  bool dg_s2 = false;   // tensor-core dgrad of a stride-2 3x3 conv as its 4 sub-pixel phases (reads dY, not zero-stuffed)
-  const float* zs = nullptr;   // fp32 mode, stride 2: the dgrad reads dY zero-stuffed to [2 out_h][2 out_w][N] instead
+  // input gradient of a stride-2 3x3 conv, read from dY at its own resolution: the tensor-core kernel runs its 4 sub-pixel
+  // phases, the SIMT kernel (fp32 mode) a stride-1 conv over dY dilated by 2
+  bool dg_s2 = false;
   float* dg_out = nullptr; int dg_out_h = 0, dg_out_w = 0; int dg_off = 0;
   // wgrad: split-K partials [part_ks][tap][128][part_cols] (the tensor-core plan gives every conv its own; the fp32-mode
   // plan shares one area between all convs), summed into the gradient by one UnpackEntry per conv
@@ -326,11 +327,11 @@ struct ConvOp {
   int part_ks(int prec) const { return is_tc(prec) ? tc_ksplits() : simt_ksplits(); }
   int part_cols(int prec) const { return is_tc(prec) ? wg_cols() : c_pad; }
   size_t partial_elems(int prec) const { return (size_t)part_ks(prec) * k * k * 128 * part_cols(prec); }
-  PackEntry pack_entry(const float* w) const {
+  PackEntry pack_entry(int prec, const float* w) const {
     PackEntry e{};
     e.w = w; e.dst_f = do_fprop ? wp_f : nullptr; e.dst_d = has_dgrad ? wp_d : nullptr;
     e.N = N; e.C = C; e.k = k; e.rot = rot; e.n_rows = Np; e.c_pad = c_pad; e.c_rows = crows;
-    e.Ctot = Ctot; e.coff = coff; e.s2 = dg_s2 ? 1 : 0;
+    e.Ctot = Ctot; e.coff = coff; e.s2 = dg_s2 && is_tc(prec) ? 1 : 0;   // (the SIMT dgrad reads flipped taps)
     e.bf16 = bf16 ? 1 : 0; e.c_pad16 = c_pad16; e.n_pad = bf16 ? n_pad16 : n_pad;
     return e;
   }
@@ -454,8 +455,7 @@ struct ConvOp {
       ENQ(rec, 1, alg_flops(), s, DIP_CUDA(tc_conv_launch(dg, g_num_sms, s)));
     } else {
       SimtConvArgs a{};
-      a.A = zs != nullptr ? zs : dy; a.a_h = zs != nullptr ? 2 * out_h : out_h; a.a_w = zs != nullptr ? 2 * out_w : out_w;
-      a.a_ld = N; a.a_c = N;
+      a.A = dy; a.a_h = out_h; a.a_w = out_w; a.a_ld = N; a.a_c = N; a.dil = dg_s2 ? 2 : 1;
       a.Wp = wp_d; a.n_rows = crows; a.c_pad = n_pad;
       a.D = dg_out; a.d_h = dg_out_h; a.d_w = dg_out_w; a.d_ld = dg_ld; a.d_c = C;
       a.kh = a.kw = k; a.stride = 1; a.offx = a.offy = dg_off; a.bias = nullptr;
@@ -561,7 +561,7 @@ struct Level {
   int Pin_ld16 = 0, cat_ld16 = 0;
   float *dUp;  // [h][w][128] adjoint of the upsampling applied to dCat
   float *dS;   // skip=128: [H][W][Cin] input gradient of the (tensor-core) skip conv, levels > 0
-  float *dRaw_v, *dA_u, *dRaw_u, *dP_cat, *dCat, *dRaw_s, *dRaw_d2, *dP_d1, *dRaw_d1, *ZS, *dPin;
+  float *dRaw_v, *dA_u, *dRaw_u, *dP_cat, *dCat, *dRaw_s, *dRaw_d2, *dP_d1, *dRaw_d1, *dPin;
   BnLayer bn_s, bn_d1, bn_d2, bn_cat, bn_u, bn_v;
   int p_skip_w, p_skip_b;
   double* dw_s;
@@ -848,8 +848,6 @@ static int build_plan(dip_plan* P, Arena& A) {
       if (bf) v.dRawF16 = b16("dRawF16", v.H, v.W, nd, nd);   // bf16 mode writes the conv's dY as the twin only
       else v.dRawF = f32("dRawF", v.H, v.W, nd, nd);
     }
-    // the exact-fp32 mode's stride-2 input gradient reads its dY zero-stuffed
-    v.ZS = (!is_tc(prec) && !avg && d1_dgrad) ? f32("ZS", v.H, v.W, nd, nd) : nullptr;
     // input gradient of the skip conv: the tensor-core 1x1 of skip=128 (levels > 0), or at level 0 the skip conv's part
     // of the network's input gradient
     v.dS = (CS > 0 && (l > 0 ? wide : d.input_grad != 0)) ? f32("dS", v.H, v.W, v.Cin, v.Cin) : nullptr;
@@ -891,13 +889,13 @@ static int build_plan(dip_plan* P, Arena& A) {
     a.out = v.raw_d1; a.out_h = v.h; a.out_w = v.w; a.stats = v.bn_d1.fwd;
     a.has_dgrad = l > 0 || d.input_grad != 0;
     a.dg_ld = v.Cin;   // level 0: stored depth (>= the conv's real input depth)
-    a.dg_s2 = is_tc(prec);   // (fp32 mode and 'avg' take the zero-stuffed stride-1 dgrad)
-    a.dy = v.dRaw_d1; a.dy16 = v.dRaw_d1_16; a.zs = a.dg_s2 ? nullptr : v.ZS;
+    a.dg_s2 = true;
+    a.dy = v.dRaw_d1; a.dy16 = v.dRaw_d1_16;
     a.dg_out = v.dPin; a.dg_out_h = v.H + 2; a.dg_out_w = v.W + 2; a.dg_off = -2;
     a.in16 = v.Pin16; a.in_ld16 = v.Pin_ld16;
     if (avg) {   // stride-1 conv at the level's full resolution; pooling is a separate pass (fwd_level / bwd_level)
       a.stride = 1; a.out = v.rawF; a.out_h = v.H; a.out_w = v.W; a.stats = nullptr;
-      a.dg_s2 = false; a.dy = v.dRawF; a.dy16 = v.dRawF16; a.zs = nullptr;
+      a.dg_s2 = false; a.dy = v.dRawF; a.dy16 = v.dRawF16;
     }
     // down2: P_d1 -> raw_d2
     ConvOp& b = v.d2;
@@ -996,9 +994,6 @@ static int build_plan(dip_plan* P, Arena& A) {
     DIP_CUDA(cudaStreamCreateWithPriority(&P->wstream, cudaStreamNonBlocking, lo));
     DIP_CUDA(cudaStreamCreateWithPriority(&P->sstream, cudaStreamNonBlocking, lo));
   }
-  // The zero-stuffed buffers are written at even positions only: clear them once.
-  for (int l = 0; l < L; ++l)
-    if (P->lv[l].ZS != nullptr) DIP_CUDA(cudaMemset(P->lv[l].ZS, 0, (size_t)P->lv[l].H * P->lv[l].W * P->lv[l].nd * sizeof(float)));
   if (is_tc(prec))
     for (ConvOp* op : P->convs) DIP_CHECK(op->build_tc());
   P->pack_max = 0;
@@ -1011,7 +1006,7 @@ static int build_plan(dip_plan* P, Arena& A) {
 
 static int upload_tables(dip_plan* P) {
   std::vector<PackEntry> pk;
-  for (ConvOp* op : P->convs) pk.push_back(op->pack_entry(P->params[op->p_w]));
+  for (ConvOp* op : P->convs) pk.push_back(op->pack_entry(P->desc.precision, P->params[op->p_w]));
   DIP_CUDA(cudaMemcpy(P->d_pack, pk.data(), pk.size() * sizeof(PackEntry), cudaMemcpyHostToDevice));
   if (P->n_unpack > 0) {
     std::vector<UnpackEntry> up;
@@ -1203,21 +1198,21 @@ static int plan_forward(dip_plan* P, const float* z, const float* noise, float s
 
 // ------------------------------------------------------------------------------------------------ backward
 static int bn_bwd(dip_plan* P, const float* raw, int ld_raw, BnLayer& b, int act, GradSrc src, int H, int W, float* draw,
-                  float* zs, cudaStream_t s, uint16_t* draw16 = nullptr) {
-  if (draw16 != nullptr && zs == nullptr) draw = nullptr;   // bf16 mode: only the tensor-core dgrad / wgrad read this gradient
+                  cudaStream_t s, uint16_t* draw16 = nullptr) {
+  if (draw16 != nullptr) draw = nullptr;   // bf16 mode: only the tensor-core dgrad / wgrad read this gradient
   if (src.kind == 1) src.zero_pad = P->zero_pad;            // zero padding: the padded gradient's halo is dropped, not folded
   BnRef r = bn_ref(P, b);
   // algorithmic bytes: raw + the gradient source as the kernel's contract names it (plain [H][W][C]; fold: the padded
   // dgrad output (+ the 4-channel skip-branch gradient / the plain addend); upsample adjoint: the 2H x 2W gradient; head:
-  // the 4 logit gradients per pixel), + the written input gradient (and its zero-stuffed copy) for the apply pass
+  // the 4 logit gradients per pixel), + the written input gradient for the apply pass
   const double px = (double)H * W, C4 = b.C * sizeof(float);
   double gsrc = px * C4;
   if (src.kind == 1) gsrc = (src.zero_pad ? px : (double)(H + 2) * (W + 2)) * C4 + (src.ds != nullptr ? px * 4 * sizeof(float) : 0.0) + (src.add != nullptr ? px * C4 : 0.0);
   else if (src.kind == 2) gsrc = 4.0 * px * C4;
   else if (src.kind == 3) gsrc = px * 4 * sizeof(float);
   ENQ(&P->rec, hbm(H_BN_BWD_REDUCE, src.kind), px * C4 + gsrc, s, launch_bn_bwd_reduce(raw, ld_raw, r, act, P->act_fun, src, H, W, b.bwd, s));
-  ENQ(&P->rec, hbm(H_BN_BWD_APPLY, src.kind + (zs != nullptr ? 4 : 0)), px * C4 + gsrc + px * C4 * (zs != nullptr ? 2.0 : 1.0), s,
-      launch_bn_bwd_apply(raw, ld_raw, r, act, P->act_fun, src, H, W, b.bwd, draw, zs, b.dbias, s, Twin{draw16, b.C}));
+  ENQ(&P->rec, hbm(H_BN_BWD_APPLY, src.kind), px * C4 + gsrc + px * C4, s,
+      launch_bn_bwd_apply(raw, ld_raw, r, act, P->act_fun, src, H, W, b.bwd, draw, b.dbias, s, Twin{draw16, b.C}));
   return 0;
 }
 static GradSrc src_plain(const float* g, int ld, int coff) { GradSrc s{}; s.kind = 0; s.g = g; s.ld = ld; s.coff = coff; return s; }
@@ -1259,11 +1254,11 @@ static int bwd_level(dip_plan* P, int l, GradSrc src_v, cudaStream_t s) {
   const int CC = v.cu + CS;
   const bool last = l == (int)P->lv.size() - 1;
   // 1x1 conv + BN + LReLU
-  DIP_CHECK(bn_bwd(P, v.raw_v, nu, v.bn_v, 1, src_v, v.H, v.W, v.dRaw_v, nullptr, s, v.dRaw_v16));
+  DIP_CHECK(bn_bwd(P, v.raw_v, nu, v.bn_v, 1, src_v, v.H, v.W, v.dRaw_v, s, v.dRaw_v16));
   if (l == kDeferLevel) DIP_CHECK(flush_deferred(P, prec, s));
   DIP_CHECK(conv_backward(P, v.c11, true, prec, s, l));
   // up conv + BN + LReLU
-  DIP_CHECK(bn_bwd(P, v.raw_u, nu, v.bn_u, 1, src_plain(v.dA_u, nu, 0), v.H, v.W, v.dRaw_u, nullptr, s, v.dRaw_u16));
+  DIP_CHECK(bn_bwd(P, v.raw_u, nu, v.bn_u, 1, src_plain(v.dA_u, nu, 0), v.H, v.W, v.dRaw_u, s, v.dRaw_u16));
   if (CS == 128) {
     cudaStream_t ws = fork_side(P, s);
     DIP_CHECK(v.up_a.run_dgrad(prec, s));
@@ -1285,7 +1280,7 @@ static int bwd_level(dip_plan* P, int l, GradSrc src_v, cudaStream_t s) {
   // gradient w.r.t. the low-resolution tensor that was upsampled into this concat (adjoint of x2 upsampling), once
   ENQ(&P->rec, hbm(H_UPADJ, v.bilinear), (double)v.cu * ((double)v.H * v.W + (double)v.h * v.w) * sizeof(float), s,
       launch_upadj(v.dCat, CC, 0, v.h, v.w, v.cu, v.bilinear, v.dUp, s));
-  if (CS > 0) DIP_CHECK(bn_bwd(P, v.raw_s, CS, v.bn_s, 1, src_plain(v.dCat, CC, v.cu), v.H, v.W, v.dRaw_s, nullptr, ks, v.dRaw_s16));
+  if (CS > 0) DIP_CHECK(bn_bwd(P, v.raw_s, CS, v.bn_s, 1, src_plain(v.dCat, CC, v.cu), v.H, v.W, v.dRaw_s, ks, v.dRaw_s16));
   if (CS == 0) {
     // no skip branch (models/skip.py:50-53 with num_channels_skip = 0)
   } else if (CS == 128) {
@@ -1310,12 +1305,12 @@ static int bwd_level(dip_plan* P, int l, GradSrc src_v, cudaStream_t s) {
   } else {
     src_d2 = src_plain(v.dUp, v.cu, 0);
   }
-  DIP_CHECK(bn_bwd(P, v.raw_d2, nd, v.bn_d2, 1, src_d2, v.h, v.w, v.dRaw_d2, nullptr, s, v.dRaw_d2_16));
+  DIP_CHECK(bn_bwd(P, v.raw_d2, nd, v.bn_d2, 1, src_d2, v.h, v.w, v.dRaw_d2, s, v.dRaw_d2_16));
   DIP_CHECK(conv_backward(P, v.d2, true, prec, s));
   const bool d1_dgrad = l > 0 || P->desc.input_grad != 0;
   const bool avg = v.rawF != nullptr;
-  DIP_CHECK(bn_bwd(P, v.raw_d1, nd, v.bn_d1, 1, src_fold(v.dP_d1, nd, nullptr, nullptr, 0), v.h, v.w, v.dRaw_d1,
-                   (d1_dgrad && !v.d1.dg_s2 && !avg) ? v.ZS : nullptr, s, avg ? nullptr : v.dRaw_d1_16));
+  DIP_CHECK(bn_bwd(P, v.raw_d1, nd, v.bn_d1, 1, src_fold(v.dP_d1, nd, nullptr, nullptr, 0), v.h, v.w, v.dRaw_d1, s,
+                   avg ? nullptr : v.dRaw_d1_16));
   if (avg)   // adjoint of AvgPool2d(2, 2): the conv's dY at full resolution
     ENQ(&P->rec, kUntimed, 0, s,
         launch_avgpool2_bwd(v.dRaw_d1, v.h, v.w, nd, prec == DIP_PRECISION_BF16 ? nullptr : v.dRawF, s, Twin{v.dRawF16, nd}));
@@ -1845,7 +1840,7 @@ static int op_setup(const char* name, ConvOp& op, int prec, const float* w, floa
     return fail(std::string(name) + ": the operands need " + std::to_string((A.off + (1 << 20) - 1) >> 20) +
                 " MB of scratch, more than dip_op_scratch_bytes() = " + std::to_string(dip_op_scratch_bytes() >> 20) + " MB");
   if (pack) {
-    const PackEntry e = op.pack_entry(w);
+    const PackEntry e = op.pack_entry(prec, w);
     DIP_CUDA(cudaMemcpyAsync(d_pack, &e, sizeof e, cudaMemcpyHostToDevice, s));
     launch_k(k_pack_table, dim3(64, 1), dim3(256), 0, s, 1, (const PackEntry*)d_pack);
   }
@@ -1886,7 +1881,6 @@ int dip_op_conv_dgrad(const void* dy, int dy_h, int dy_w, const void* w, int N, 
 }
 int dip_op_conv_dgrad_s2(const void* dy, int dy_h, int dy_w, const void* w, int N, int C, int rot, void* dx, int precision,
                          void* scratch, dip_stream_t stream) {
-  if (!is_tc(precision)) return fail("dip_op_conv_dgrad_s2: tensor-core path only (the exact-fp32 mode zero-stuffs)");
   cudaStream_t s = (cudaStream_t)stream;
   ConvOp op;
   op.N = N; op.C = C; op.k = 3; op.stride = 2; op.rot = rot;

@@ -168,13 +168,12 @@ void launch_input_grad(const float* gp, const float* ds, int ld, int C, int H, i
 
 // BN(+activation) backward. reduce: bwd[0..C) += sum dz, bwd[C..2C) += sum dz*xhat.
 // dz = f'(y) * gradient (act != 0; f = act_fun, y = the pre-activation, recomputed from raw) or the gradient itself.
-// apply: dx = gamma*rstd*(dz - mean(dz) - xhat*mean(dz*xhat)); writes draw plain [H][W][C];
-//        optionally a zero-stuffed copy zs [2H][2W][C] (only even positions written); dbias[c] += sum dx.
+// apply: dx = gamma*rstd*(dz - mean(dz) - xhat*mean(dz*xhat)); writes draw plain [H][W][C]; dbias[c] += sum dx.
 void launch_bn_bwd_reduce(const float* raw, int ld_raw, BnRef bn, int act, int act_fun, GradSrc src, int H, int W,
                           double* bwd, cudaStream_t s);
 // draw may be null when a bf16 twin is given
 void launch_bn_bwd_apply(const float* raw, int ld_raw, BnRef bn, int act, int act_fun, GradSrc src, int H, int W,
-                         const double* bwd, float* draw, float* zs, double* dbias, cudaStream_t s, Twin t16 = kNoTwin);
+                         const double* bwd, float* draw, double* dbias, cudaStream_t s, Twin t16 = kNoTwin);
 
 // In-net 'avg' downsampling (models/common.py:101-105: conv stride 1 + nn.AvgPool2d(2, 2)): y[i][j][c] = mean of the 2 x 2 block
 // of x [2h][2w][C]; its adjoint spreads 0.25 * dy to the four positions (optionally also as a bf16 twin; dx may be null then)
@@ -284,6 +283,8 @@ struct SimtConvArgs {
   float* D; int d_h, d_w, d_ld, d_c;             // output NHWC
   int kh, kw, stride, offx, offy;
   const float* bias;
+  int dil = 1;                                   // input dilation (1 or 2): the input the kernel convolves is
+                                                 // (dil*a_h) x (dil*a_w), A[i][j] at (dil*i, dil*j) and zeros between
 };
 void launch_simt_conv(SimtConvArgs a, cudaStream_t s);
 struct SimtWgradArgs {

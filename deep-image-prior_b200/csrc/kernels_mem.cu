@@ -877,7 +877,7 @@ void launch_bn_bwd_reduce(const float* raw, int ld_raw, BnRef bn, int act, int a
 template <int KIND, bool ZP = false, int ACT = kActLeakyRelu>
 __global__ void __launch_bounds__(256, KIND == 2 ? 3 : 2) k_bn_bwd_apply(const float* __restrict__ raw, int ld_raw, BnRef bn, int act, GradSrc src,
                                                       int H, int W, const double* __restrict__ bwd, float* __restrict__ draw,
-                                                      float* __restrict__ zs, double* __restrict__ dbias, int VL, int PPB, Twin t16) {
+                                                      double* __restrict__ dbias, int VL, int PPB, Twin t16) {
   pdl_enter();
   const int v = threadIdx.x % VL, slot = threadIdx.x / VL;
   const Bn4 cf = bn_coef<0>(bn, v);
@@ -904,7 +904,6 @@ __global__ void __launch_bounds__(256, KIND == 2 ? 3 : 2) k_bn_bwd_apply(const f
                            dx.w = cf.scale.w * (dz.w - m1.w - xh.w * m2.w);
                            if (draw != nullptr) st4(draw + (static_cast<size_t>(i) * W + j) * C + 4 * v, dx);
                            if (t16.p != nullptr) st4_bf16(t16.p + (static_cast<size_t>(i) * W + j) * t16.ld + 4 * v, dx);
-                           if (zs != nullptr) st4(zs + (static_cast<size_t>(2 * i) * (2 * W) + 2 * j) * C + 4 * v, dx);
                            acc[0] = f4add(acc[0], dx);
                          });
   } else
@@ -938,10 +937,6 @@ __global__ void __launch_bounds__(256, KIND == 2 ? 3 : 2) k_bn_bwd_apply(const f
         dx.w = cf.scale.w * (dz.w - m1.w - xh.w * m2.w);
         if (draw != nullptr) st4(draw + static_cast<size_t>(p) * C + 4 * v, dx);
         if (t16.p != nullptr) st4_bf16(t16.p + static_cast<size_t>(p) * t16.ld + 4 * v, dx);
-        if (zs != nullptr) {
-          const int i = p / W, j = p - i * W;
-          st4(zs + (static_cast<size_t>(2 * i) * (2 * W) + 2 * j) * C + 4 * v, dx);
-        }
         acc[0] = f4add(acc[0], dx);
       });
   if constexpr (KIND == 3) {
@@ -957,7 +952,7 @@ __global__ void __launch_bounds__(256, KIND == 2 ? 3 : 2) k_bn_bwd_apply(const f
   }
 }
 void launch_bn_bwd_apply(const float* raw, int ld_raw, BnRef bn, int act, int act_fun, GradSrc src, int H, int W,
-                         const double* bwd, float* draw, float* zs, double* dbias, cudaStream_t s, Twin t16) {
+                         const double* bwd, float* draw, double* dbias, cudaStream_t s, Twin t16) {
   VecGeom g = vec_geom(bn.C, static_cast<long long>(H) * W);
   const size_t sm = red_bytes(g, src.kind == 3 ? 6 : 1);
   auto kernel = act_pick(act_fun, [&](auto a) {
@@ -967,7 +962,7 @@ void launch_bn_bwd_apply(const float* raw, int ld_raw, BnRef bn, int act, int ac
          : src.kind == 2 ? k_bn_bwd_apply<2, false, A> : k_bn_bwd_apply<3, false, A>;
   });
   fit_grid(g, kernel, sm);
-  launch_red(kernel, g.blocks, g.threads, sm, s, raw, ld_raw, bn, act, src, H, W, bwd, draw, zs, dbias, g.VL, g.PPB, t16);
+  launch_red(kernel, g.blocks, g.threads, sm, s, raw, ld_raw, bn, act, src, H, W, bwd, draw, dbias, g.VL, g.PPB, t16);
 }
 
 // ------------------------------------------------------------------------------------------------ concat-BN backward

@@ -202,9 +202,10 @@ int dip_op_conv_fprop(const void* a, int a_h, int a_w, int a_c, const void* w, c
 int dip_op_conv_dgrad(const void* dy, int dy_h, int dy_w, const void* w, int N, int C, int k, int rot, void* dx,
                       int dx_h, int dx_w, int precision, void* scratch, dip_stream_t stream);
 /* Input gradient of a 3x3 STRIDE-2 convolution (the adjoint that autograd runs for the down-sampling convs,
- * models/skip.py:64 / models/common.py:120; = ConvTranspose2d(stride 2)), computed as its four sub-pixel phases -- no
- * zero-stuffing: dx[(2*dy_h+2)][(2*dy_w+2)][C], dx[u][v][c] = sum_{r = u mod 2 .. , s = v mod 2 ..} dy[(u-r)/2][(v-s)/2][n]
- * w[n][(c+rot)%C][r][s]  (every element of dx is written; tensor-core path only). */
+ * models/skip.py:64 / models/common.py:120; = ConvTranspose2d(stride 2)), read from dy at its own resolution (tensor
+ * cores: its four sub-pixel phases; precision fp32: a stride-1 conv over dy dilated by 2):
+ * dx[(2*dy_h+2)][(2*dy_w+2)][C], dx[u][v][c] = sum_{r = u mod 2 .. , s = v mod 2 ..} dy[(u-r)/2][(v-s)/2][n]
+ * w[n][(c+rot)%C][r][s]  (every element of dx is written). */
 int dip_op_conv_dgrad_s2(const void* dy, int dy_h, int dy_w, const void* w, int N, int C, int rot, void* dx, int precision,
                          void* scratch, dip_stream_t stream);
 /* dw[n][(c+rot)%C][r][s] = sum dy[y][x][n] * a[y*stride+offy+r][x*stride+offx+s][c] */

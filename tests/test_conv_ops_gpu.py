@@ -109,12 +109,13 @@ def test_wgrad(case, prec):
     assert err < TOL[prec], err
 
 
-@pytest.mark.parametrize("prec", [0, 2])
+@pytest.mark.parametrize("prec", [1, 0, 2])
 @pytest.mark.parametrize("case", [(128, 16, 16), (128, 64, 64), (128, 129, 128), (32, 40, 24), (128, 9, 13), (128, 2, 2)])
 def test_dgrad_stride2_phases(case, prec):
-    """Input gradient of the 3x3 stride-2 convs as four sub-pixel phase GEMMs in one launch (no zero-stuffing), vs
-    conv_transpose2d(stride=2) in fp64.  dx is the padded (2h+2) x (2w+2) gradient: the transposed conv covers
-    (2h+1) x (2w+1), the last row / column receive no tap and must come out as exact zeros (never left unwritten)."""
+    """Input gradient of the 3x3 stride-2 convs read from dY at its own resolution (tensor cores: four sub-pixel phase
+    GEMMs in one launch; fp32: the SIMT kernel over dY dilated by 2), vs conv_transpose2d(stride=2) in fp64.  dx is the
+    padded (2h+2) x (2w+2) gradient: the transposed conv covers (2h+1) x (2w+1), the last row / column receive no tap and
+    must come out as exact zeros (never left unwritten)."""
     import dip_engine as de
     C, h, w_ = case
     g = torch.Generator().manual_seed(4)

@@ -30,10 +30,6 @@ LEVEL_BUFFERS = ["Pin", "raw_s", "raw_d1", "rawF", "P_d1", "raw_d2", "P_d2", "P_
                  "dRaw_v", "dA_u", "dRaw_u", "dP_cat", "dCat", "dRaw_s", "dUp", "dS", "dRaw_d2", "dP_d1", "dRaw_d1",
                  "dRawF", "dPin", "Pin16", "P_d1_16", "P_d2_16", "P_cat16", "A_u16", "dRaw_v16", "dRaw_u16", "dRaw_d2_16",
                  "dRaw_d1_16", "dRaw_s16", "dRawF16"]
-# (not "ZS": the zero-stuffed dY of the exact-fp32 stride-2 input gradient.  The BN backward writes its even positions
-# only (k_bn_bwd_apply in kernels_mem.cu, the `zs` store), and the odd ones keep the zeros that build_plan writes once
-# when dip_plan_create builds the plan: the cudaMemset of every level's ZS after "The zero-stuffed buffers are written
-# at even positions only: clear them once" in engine.cu.)
 WORST = {}   # mode -> {stage: worst |err| / tolerance}
 FROB = {}    # mode -> {conv stage: worst relative Frobenius error / its bound}
 
